@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — Mrays/s of the NeRFshop render path at 1920x1080 on the synthetic nerf/fox-shaped workload.
 
-  python bench.py --gpus N --steps K --warmup W [--impl native|reference]
+  python bench.py --gpus N --steps K --warmup W [--impl native|reference] [--dump-outputs DIR]
 
 A "step" is one frame: Testbed::render_nerf of one camera of a 120-view orbit (a different camera every
 step = free-viewpoint orbit), base.json network (hash L=16 F=2 T=2^19, MLPs 64x1 / 64x2), synthetic seeded
@@ -15,8 +15,11 @@ e2e.value  : the same with every frame delivered to pinned HOST memory inside th
 roofline   : the one kernel of the step (k_render_fused): algorithmic 512 B hash-grid gather per sample
              (SURVEY.md §8d) x samples of the frame / its CUDA-event duration, against measured HBM peak
 gpu_baseline: (N = 1) the reference's OWN CUDA path — Testbed::render_nerf, NerfTracer::trace and every kernel they launch, compiled
-             by nvcc for sm_100a from /root/reference (oracle/_ref, built where the reference exists; only tiny-cuda-nn's network, an
+             by nvcc for sm_90a from the reference's sources (oracle/_ref, built where the reference exists; only tiny-cuda-nn's network, an
              absent submodule, is replaced by this repository's nsb_inference) — timed in the same process on the same cameras.
+--dump-outputs DIR: after the timed steps, the last timed step's frame as DIR/rgba.npy (float32 [H, W, 4]) and DIR/depth.npy
+             (float32 [H, W]); --impl reference writes its last CPU frame the same way. Inputs are seeded: the same arguments give the
+             same inputs on every run, so two builds can be compared output for output.
 configs    : (N = 1) BASELINE.json configs[2] (one cage, 3,072 tets) and configs[3] (unit-cube scene, 3 cages + membrane, poisson target)
              at 1920x1080: native and reference-CUDA Mrays/s, samples, roofline fraction, L-inf between the two.
 cpu_baseline / --impl reference: the reference's Testbed::render_nerf compiled for the CPU (oracle/_ref/libnerfshop_ref.so: its own host
@@ -56,22 +59,6 @@ def emit(line: str) -> None:
     out.flush()
 
 
-def load_traffic():
-    """DRAM bytes per launch of k_render_fused from the committed `ncu --set full` digest (profiles/), or None."""
-    import glob
-    import re
-
-    best = None
-    for path in sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_ncu_render_fused*.txt"))):
-        txt = open(path).read()
-        rd = re.search(r"dram__bytes_read\.sum\s+([0-9.]+)\s+(\w+)", txt)
-        wr = re.search(r"dram__bytes_write\.sum\s+([0-9.]+)\s+(\w+)", txt)
-        if rd and wr:
-            scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-            best = (float(rd.group(1)) * scale.get(rd.group(2), 1.0) + float(wr.group(1)) * scale.get(wr.group(2), 1.0), os.path.basename(path))
-    return best
-
-
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -80,11 +67,11 @@ def load_peaks():
             return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0))), "measured"
         except Exception:
             pass
-    return 6650.0, 1590.0, "fallback"
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -133,7 +120,7 @@ class ClockSampler:
 def cpu_reference_run(steps: int, warmup: int, threads: int | None = None):
     """The CPU arm: the reference's own render_nerf compiled for the CPU (oracle/_ref) when available, else the oracle port.
     All host cores, threads pinned (OMP_PROC_BIND / OMP_PLACES are set by main() before any OpenMP runtime starts), bounded sample per step.
-    Returns (Mrays/s from the MEDIAN step, median ms, cores, samples per frame, kind, (p10, p90) ms)."""
+    Returns (Mrays/s from the MEDIAN step, median ms, cores, samples per frame, kind, (p10, p90) ms, last step's (rgba, depth))."""
     from nerfshop_b200 import synthetic as syn
     from oracle import oracle as orc
 
@@ -156,10 +143,10 @@ def cpu_reference_run(steps: int, warmup: int, threads: int | None = None):
         f = syn.make_frame(model, cams[(i * 7) % N_ORBIT], CPU_W, CPU_H)
         t0 = time.perf_counter()
         if ref is not None:
-            _, _, info = ref.render(f, occ, o.inference)
+            rgba, depth, info = ref.render(f, occ, o.inference)
             n = info["n_inferred"] // 2  # the reference infers every (padded) batch twice
         else:
-            _, _, st, _ = o.render(f)
+            rgba, depth, st, _ = o.render(f)
             n = st.n_samples
         dt = time.perf_counter() - t0
         if i >= warmup:
@@ -167,11 +154,19 @@ def cpu_reference_run(steps: int, warmup: int, threads: int | None = None):
             samples += n
     med = float(np.median(times))
     mrays = CPU_W * CPU_H / med / 1e6
-    return mrays, med * 1e3, cores, samples / max(len(times), 1), kind, (float(np.percentile(times, 10)) * 1e3, float(np.percentile(times, 90)) * 1e3)
+    return (mrays, med * 1e3, cores, samples / max(len(times), 1), kind, (float(np.percentile(times, 10)) * 1e3, float(np.percentile(times, 90)) * 1e3),
+            (np.asarray(rgba), np.asarray(depth)))
+
+
+def dump_outputs(out_dir: str, rgba, depth) -> None:
+    """The frame a caller of the timed path receives: RGBA [H, W, 4] and depth [H, W], float32."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "rgba.npy"), np.ascontiguousarray(rgba, dtype=np.float32))
+    np.save(os.path.join(out_dir, "depth.npy"), np.ascontiguousarray(depth, dtype=np.float32))
 
 
 def measure_reference_cuda_and_edit_configs(r, model, occ, cams, fb, depth, flush, steps, dev):
-    """N = 1 only. (1) gpu_baseline: the reference's CUDA path (oracle/_ref, nvcc build of /root/reference's render path; network = nsb_inference)
+    """N = 1 only. (1) gpu_baseline: the reference's CUDA path (oracle/_ref, nvcc build of the reference's render path; network = nsb_inference)
     on the orbit cameras of configs[1]. (2) configs[2] / configs[3] at 1080p, native and reference-CUDA. CUDA events around each frame, L2 flushed
     between frames, 3 warm-up frames, median over the timed frames (both arms)."""
     import torch
@@ -183,7 +178,7 @@ def measure_reference_cuda_and_edit_configs(r, model, occ, cams, fb, depth, flus
         from oracle import ref
 
         ref.cuda_lib()
-    except Exception as e:  # the library is built where /root/reference exists and travels with the repo
+    except Exception as e:  # the library is built where the reference's sources exist
         return {"unavailable": f"oracle/_ref/libnerfshop_ref_cuda.so not loadable: {e}"}, None
 
     def time_frames(render_fn, frames, n):
@@ -225,12 +220,12 @@ def measure_reference_cuda_and_edit_configs(r, model, occ, cams, fb, depth, flus
         }
 
     what = ("the reference's own CUDA render path (Testbed::render_nerf, NerfTracer::trace, compact/generate/composite/shade kernels; >= 12 launches + 3 host syncs per round, "
-            "every batch inferred twice) compiled by nvcc for sm_100a from /root/reference; tiny-cuda-nn's network (absent submodule) replaced by this repository's nsb_inference kernel")
+            "every batch inferred twice) compiled by nvcc for sm_90a from the reference's sources; tiny-cuda-nn's network (absent submodule) replaced by this repository's nsb_inference kernel")
     frames = [syn.make_frame(model, cams[(i * 7) % N_ORBIT], W, H) for i in range(steps)]
     rc = ref.RefCuda(occ)
     res = both_arms(r, rc, frames, steps)
     rc.close()
-    gpu_baseline = dict(res["reference_cuda"], kind="reference kernels + host loop, nvcc sm_100a", what=what, native_ms_same_cameras=res["native"]["ms_per_step"],
+    gpu_baseline = dict(res["reference_cuda"], kind="reference kernels + host loop, nvcc sm_90a", what=what, native_ms_same_cameras=res["native"]["ms_per_step"],
                         linf_rgba_native_vs_reference_cuda_frame0=res["linf_rgba_native_vs_reference_cuda_frame0"], steps=steps, warmup=3)
 
     extra = {}
@@ -240,7 +235,7 @@ def measure_reference_cuda_and_edit_configs(r, model, occ, cams, fb, depth, flus
     r.set_edit_operators(ops)
     rc = ref.RefCuda(occ, ops)
     fr = [syn.make_frame(model, cams[(i * 7) % N_ORBIT], W, H, apply_operators=True) for i in range(4)]
-    extra["configs[2]"] = dict(both_arms(r, rc, fr, 6), workload=f"nerf/fox scale, one cage ({cage.tets.shape[0]} tets, {cage.lut_idx.size} CSR entries), 1080p, 4 orbit cameras")
+    extra["configs[2]"] = dict(both_arms(r, rc, fr, steps), workload=f"nerf/fox scale, one cage ({cage.tets.shape[0]} tets, {cage.lut_idx.size} CSR entries), 1080p, 4 orbit cameras")
     rc.close()
     r.set_edit_operators([])
     # configs[3]: unit-cube scene (aabb_scale 1, cone angle 0: the reference's synthetic-Lego shape), 3 concurrent cages (6^3 lattices), membrane on the first, poisson target on
@@ -256,7 +251,7 @@ def measure_reference_cuda_and_edit_configs(r, model, occ, cams, fb, depth, flus
     r1.set_edit_operators(ops)
     rc = ref.RefCuda(occ1, ops)
     fr = [syn.make_frame(m1, cams[(i * 7) % N_ORBIT], W, H, apply_operators=True, poisson_target=True) for i in range(4)]
-    extra["configs[3]"] = dict(both_arms(r1, rc, fr, 6), workload=f"unit-cube scene (aabb_scale 1, constant step), 3 cages ({sum(c.tets.shape[0] for c in cages)} tets) + membrane + poisson target, 1080p, 4 orbit cameras")
+    extra["configs[3]"] = dict(both_arms(r1, rc, fr, steps), workload=f"unit-cube scene (aabb_scale 1, constant step), 3 cages ({sum(c.tets.shape[0] for c in cages)} tets) + membrane + poisson target, 1080p, 4 orbit cameras")
     rc.close()
     r1.close()
     return gpu_baseline, extra
@@ -270,6 +265,7 @@ def main():
     ap.add_argument("--impl", default="native", choices=["native", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-baseline", action="store_true", help="skip the reference-CUDA arm and the edit configurations (N = 1 extras)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's frame (rgba.npy, depth.npy; float32) to DIR")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -295,11 +291,13 @@ def main():
     if args.impl == "reference":
         if rank != 0:
             return
-        steps = max(1, min(args.steps, 8))
-        warm = max(3, min(args.warmup, 3))
-        mrays, ms, cores, spf, kind, (p10, p90) = cpu_reference_run(steps, warm)
+        steps = max(1, args.steps)
+        warm = max(0, args.warmup)
+        mrays, ms, cores, spf, kind, (p10, p90), last = cpu_reference_run(steps, warm)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, *last)
         sample = f"{CPU_W}x{CPU_H} frame (1/64 of the 1080p pixels) of the same orbit per step, {cores} pinned threads, median of {steps} steps (p10 {p10:.0f} ms, p90 {p90:.0f} ms), {warm} warm-up"
-        note = ("the reference's Testbed::render_nerf / NerfTracer::trace / kernels compiled for the CPU from /root/reference (oracle/_ref); tiny-cuda-nn's network (absent submodule) = the oracle's CPU restatement"
+        note = ("the reference's Testbed::render_nerf / NerfTracer::trace / kernels compiled for the CPU from its sources (oracle/_ref); tiny-cuda-nn's network (absent submodule) = the oracle's CPU restatement"
                 if kind == "reference" else "CPU oracle port of the reference path (oracle/_ref/libnerfshop_ref.so not present)")
         emit(json.dumps({
             "impl": "reference", "metric": METRIC, "value": mrays, "unit": "Mrays/s", "n_gpus": 0, "steps": steps, "warmup": warm,
@@ -335,7 +333,7 @@ def main():
     if world > 1:
         shard = torch.zeros(max_tiles * 128 * 5, dtype=torch.float32, device=dev)            # [tiles*128 float4 | tiles*128 depth]
         gathered = torch.zeros((world, max_tiles * 128 * 5), dtype=torch.float32, device=dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
     host_fb = torch.zeros((H, W, 4), dtype=torch.float32).pin_memory()
     host_depth = torch.zeros((H, W), dtype=torch.float32).pin_memory()
     stream = torch.cuda.current_stream(dev)
@@ -385,6 +383,8 @@ def main():
         sampler.start()
     total_ms, wall, kern_ms, samples = timed(device_step, args.warmup, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:  # before the e2e and baseline legs reuse the framebuffer
+        dump_outputs(args.dump_outputs, fb.cpu().numpy(), depth.cpu().numpy())
 
     # ---- e2e: every step's frame ends in (pinned) HOST memory; the copy of frame k overlaps the render of frame k+1, two frames in flight ----
     # N = 1: the C ABI's host-buffer entry point nsb_render_host_async / nsb_host_frame_wait (the consumer takes frame k-1 while frame k renders).
@@ -444,11 +444,10 @@ def main():
     # ---- N = 1 extras: the reference's own CUDA path on the same cameras, and the edit configurations ----
     gpu_baseline, extra_configs = None, None
     if world == 1 and not args.no_gpu_baseline:
-        gpu_baseline, extra_configs = measure_reference_cuda_and_edit_configs(r, model, occ, cams, fb, depth, flush, min(args.steps, 8), dev)
+        gpu_baseline, extra_configs = measure_reference_cuda_and_edit_configs(r, model, occ, cams, fb, depth, flush, args.steps, dev)
 
     if rank == 0:
         hbm_gbs, tflops, peak_kind = load_peaks()
-        traffic = load_traffic()
         ms_per_step = total_ms / args.steps
         value = W * H / (ms_per_step * 1e-3) / 1e6
         e2e_value = W * H * args.steps / e2e_s / 1e6
@@ -457,7 +456,7 @@ def main():
         achieved = s_mean * BYTES_PER_SAMPLE / (k_ms * 1e-3) / 1e9
         out = {
             "metric": METRIC, "value": value, "unit": "Mrays/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
-            "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f16 (hash features, MLP operands and tcgen05 accumulators, as the reference's wmma half fragments; fp32 march / deform / composite)",
+            "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f16 (hash features, MLP operands and wgmma accumulators, as the reference's wmma half fragments; fp32 march / deform / composite)",
             "data": "synthetic", "fps": 1e3 / ms_per_step,
             "config": dict(config, l2="flushed between timed steps (256 MiB memset outside the per-step event bracket)",
                            samples_per_frame=s_mean * world, samples_per_ray=s_mean * world / (W * H)),
@@ -466,7 +465,7 @@ def main():
                     "d2h_bytes_per_step": W * H * 20, "ms_per_step": e2e_s / args.steps * 1e3},
             "gpu_launches": launches_per_step * args.steps,
             "roofline": {"kernel": "k_render_fused", "bound": "hbm", "achieved": achieved, "peak": hbm_gbs, "unit": "GB/s", "frac": achieved / hbm_gbs,
-                         "traffic": traffic[0] if traffic else None, "traffic_source": traffic[1] if traffic else None, "peak_source": peak_kind, "kernel_ms": k_ms, "kernel_share_of_step": k_ms / ms_per_step if world == 1 else None, "samples_per_launch": s_mean,
+                         "peak_source": peak_kind, "kernel_ms": k_ms, "kernel_share_of_step": k_ms / ms_per_step if world == 1 else None, "samples_per_launch": s_mean,
                          "tensor_tflops": s_mean * FLOP_PER_SAMPLE / (k_ms * 1e-3) / 1e12, "tensor_frac": s_mean * FLOP_PER_SAMPLE / (k_ms * 1e-3) / 1e12 / tflops},
         }
         if world == 1:
@@ -475,7 +474,7 @@ def main():
                 out["vs_gpu_baseline"] = {"device": value / gpu_baseline["value"], "north_star_target": 1.5}
             out["configs"] = extra_configs
         if world == 1 and not args.no_cpu_baseline:
-            mrays, ms, cores, _, kind, (p10, p90) = cpu_reference_run(3, 1)
+            mrays, ms, cores, _, kind, (p10, p90), _ = cpu_reference_run(3, 1)
             out["cpu_baseline"] = {"value": mrays, "unit": "Mrays/s", "cores": cores, "kind": kind,
                                    "sample": f"median of 3 frames of {CPU_W}x{CPU_H} (1/64 of the 1080p pixels) of the same orbit after 1 warm-up, {cores} pinned threads (p10 {p10:.0f} / p90 {p90:.0f} ms)"}
         emit(json.dumps(out))

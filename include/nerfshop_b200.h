@@ -1,5 +1,5 @@
 /*
- * nerfshop_b200.h — C ABI of the B200-native NeRFshop render path.
+ * nerfshop_b200.h — C ABI of the H100-native NeRFshop render path.
  *
  * This is the drop-in boundary for ONE hot path of graphdeco-inria/nerfshop:
  *   Testbed::render_nerf            (reference src/testbed_nerf.cu:3066-3201)
@@ -215,8 +215,8 @@ NsbStatus nsb_model_n_params(const NsbModelDesc* desc, uint64_t* n_params);
 NsbStatus nsb_upload_model(NsbContext* ctx, const NsbModelDesc* desc, const uint16_t* params_fp16, uint64_t n_params);
 /* Accumulator policy of the two fully fused MLPs (every entry point that evaluates the network). The reference's tiny-cuda-nn FullyFusedMLP
  * runs wmma m16n16k16 with __half accumulator fragments (SURVEY.md Appendix B; the submodule is absent, so this is not verifiable here):
- *   NSB_MLP_ACC_F16 (default) fp16 accumulators in TMEM: the running sum is rounded to fp16 by every K=16 tcgen05.mma, as with __half fragments;
- *   NSB_MLP_ACC_F32 fp32 accumulators in TMEM, one rounding to fp16 per layer output (more accurate, not what the reference computes).
+ *   NSB_MLP_ACC_F16 (default) fp16 accumulators: the running sum is rounded to fp16 by every K=16 wgmma, as with __half fragments;
+ *   NSB_MLP_ACC_F32 fp32 accumulators, one rounding to fp16 per layer output (more accurate, not what the reference computes).
  * The two differ by up to 1e-2 in RGBA on 0.02 % of the pixels of a 480x270 frame (tests/test_mlp_policy.py, DESIGN.md section 3). */
 typedef enum { NSB_MLP_ACC_F32 = 0, NSB_MLP_ACC_F16 = 1 } NsbMlpAccumulator;
 NsbStatus nsb_set_mlp_accumulator(NsbContext* ctx, int32_t policy);

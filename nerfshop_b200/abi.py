@@ -1,6 +1,6 @@
 """ctypes mirror of include/nerfshop_b200.h (the C ABI) and the loader of the CUDA library.
 
-The product path has NO CPU fallback: `load_library()` raises if the sm_100a shared
+The product path has NO CPU fallback: `load_library()` raises if the sm_90a shared
 library has not been built (`python -c "import __graft_entry__ as g; g.build()"`).
 """
 from __future__ import annotations
@@ -153,7 +153,7 @@ def load_library(path: str | None = None) -> C.CDLL:
     p = path or os.environ.get("NSB_LIB_PATH") or LIB_PATH  # NSB_LIB_PATH: A/B builds of the same library
     if not os.path.exists(p):
         raise NsbError(
-            f"{p} not found: build the sm_100a extension first (python -c 'import __graft_entry__ as g; g.build()'). "
+            f"{p} not found: build the sm_90a extension first (python -c 'import __graft_entry__ as g; g.build()'). "
             "nerfshop_b200 has no CPU fallback."
         )
     lib = C.CDLL(p)

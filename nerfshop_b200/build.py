@@ -1,4 +1,4 @@
-"""Builds nerfshop_b200/lib/libnerfshop_b200.so (hand-written sm_100a CUDA + host C++), in-tree.
+"""Builds nerfshop_b200/lib/libnerfshop_b200.so (hand-written sm_90a CUDA + host C++), in-tree.
 
 nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box with the repo snapshot.
 """
@@ -16,7 +16,7 @@ SOURCES = ["nsb_kernels.cu", "nsb_host_geometry.cpp"]
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h", ".hpp"))) + [
     os.path.join("..", "..", "include", "nerfshop_b200.h"), os.path.join("..", "host", "nerfshop_host.hpp")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fno-fast-math", "-shared",
 ]
 

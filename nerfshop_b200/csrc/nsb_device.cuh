@@ -1,4 +1,4 @@
-// nsb_device.cuh — device functions of the render path (sm_100a).
+// nsb_device.cuh — device functions of the render path (sm_90a).
 //
 // Every fp32 operation that feeds a sample position, a grid index or an fp16 rounding is pinned with
 // explicit round-to-nearest intrinsics (__fmul_rn/__fadd_rn/__fmaf_rn/__fdiv_rn) so that ptxas cannot
@@ -37,7 +37,7 @@ struct DevLevel {
 struct DevModel {
 	DevLevel levels[MAX_LEVELS];
 	const __half2* grid;      // hash-grid entries
-	const uint8_t* w_image;   // 20480-byte shared-memory image of the 5 weight matrices (UMMA B layout)
+	const uint8_t* w_image;   // 20480-byte shared-memory image of the 5 weight matrices (wgmma B layout)
 	const __half* w_rowmajor; // the same weights, reference order (row-major per layer), for debugging kernels
 	uint32_t n_levels;
 	uint32_t pair_mode[MAX_LEVELS / 2];  // per pair of levels: 0 both dense, 1 both hashed, 2 mixed
@@ -558,8 +558,6 @@ __device__ __forceinline__ uint32_t grid_index(const DevLevel& L, uint32_t gx, u
 
 // NL consecutive levels at once: all 8*NL gathers are issued before the first one is consumed (memory-level parallelism;
 // the walk is bound by L1/L2 gather throughput, not by arithmetic).
-// (Measured and rejected, profiles/README.md: fetching x-neighbour corner pairs with one 8-byte load when they share
-// an aligned slot — the extra index arithmetic and predication cost more than the ~25% fewer gathers saved.)
 template <int NL, int MODE>
 __device__ __forceinline__ void encode_levels(const DevLevel* __restrict__ L, const __half2* __restrict__ grid, float x, float y, float z, __half2* out) {
 	__half2 v[NL][8];

@@ -1,9 +1,9 @@
-// nsb_kernels.cu — kernels of the B200-native NeRFshop render path and the C ABI on top of them.
+// nsb_kernels.cu — kernels of the H100-native NeRFshop render path and the C ABI on top of them.
 //
 // The product kernel is k_render_fused: ONE persistent launch per frame that replaces the reference's
 // per-round pipeline (compact -> generate inputs -> [residuals] -> inference -> [map_rays] -> inference ->
 // composite, >= 12 launches + 3 host syncs per round, testbed_nerf.cu:2812-2990) and its 4.6 GB of
-// scratch: ray state lives in registers and shared memory, samples go march -> deform -> hash encode -> tcgen05 MLP ->
+// scratch: ray state lives in registers and shared memory, samples go march -> deform -> hash encode -> wgmma MLP ->
 // composite without touching HBM, and finished rays are shaded straight into the framebuffer.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -118,9 +118,8 @@ __global__ void __launch_bounds__(256) k_prepare_rays(const DevFrame f, const ui
 }
 
 // grid features of one sample -> this thread's row of the A operand (4 chunks x 8 fp16)
-// Code size matters here: the fused kernel's hot loop has to live in the SM's instruction cache (profiles/README.md:
-// the first, fully unrolled version was 504 KB of SASS and stalled on instruction fetch). One loop body = 2 levels
-// (16 gathers in flight per thread), 8 iterations.
+// Code size matters here: the fused kernel's hot loop has to live in the SM's instruction cache (a fully unrolled version
+// stalls on instruction fetch). One loop body = 2 levels (16 gathers in flight per thread), 8 iterations.
 #ifndef NSB_ENC_NL
 #define NSB_ENC_NL 2  // levels per loop iteration (8*NL gathers in flight per thread)
 #endif
@@ -139,7 +138,7 @@ __device__ __forceinline__ void encode_to_a32(uint8_t* a32, const DevModel& m, b
 			else encode_levels<NL, 2>(m.levels + NL * g, m.grid, pw.x, pw.y, pw.z, h);
 		}
 		// levels NL*g .. NL*g+NL-1 = fp16 features 2*NL*g ..: NL*4 bytes of this row's k-chunk (NL*g)/4
-		uint8_t* dst = a32 + ((NL * g) >> 2) * (tc::ROWS * 16) + row * 16 + ((NL * g) & 3) * 4;
+		uint8_t* dst = a32 + ((NL * g) >> 2) * (tc::ROWS * 16) + tc::phys_row(row) * 16 + ((NL * g) & 3) * 4;
 		if (NL == 2) *reinterpret_cast<uint2*>(dst) = make_uint2(tc::pack_h2(h[0]), tc::pack_h2(h[1]));
 		else *reinterpret_cast<uint4*>(dst) = make_uint4(tc::pack_h2(h[0]), tc::pack_h2(h[1]), tc::pack_h2(h[NL > 2 ? 2 : 0]), tc::pack_h2(h[NL > 3 ? 3 : 0]));
 	}
@@ -160,19 +159,18 @@ __device__ __forceinline__ uint32_t nth_set_bit(uint32_t m, uint32_t k) {
 }
 
 // Stage 2 (persistent; a tile = 128 threads = 128 ray slots = 128 MMA rows, NSB_TILES tiles per CTA): every round each live ray contributes
-// ONE sample; samples go deform -> hash encode -> tcgen05 MLPs -> composite inside the SM; a finished ray is shaded
+// ONE sample; samples go deform -> hash encode -> wgmma MLPs -> composite inside the SM; a finished ray is shaded
 // into the framebuffer and its slot refilled from the queue (warp-convergent fetch of consecutive entries, so rays that
 // were refilled together — neighbouring pixels that die on the same surface — stay together in a warp).
 // Per-slot ray state parked in shared memory (SoA: lane-contiguous, conflict-free). Only the acquire and composite phases
 // touch it, so it does not occupy registers while the thread gathers hash-grid features and walks the MLP layers.
 enum { R_OX = 0, R_OY, R_OZ, R_DX, R_DY, R_DZ, R_T, R_CR, R_CG, R_CB, R_CA, R_DEPTH, R_MAXW, R_FIELDS };
-// One CTA per SM holds NSB_TILES independent tiles (a tile = 128 threads = 128 ray slots = one UMMA M). The tiles share the 20 KB
+// One CTA per SM holds NSB_TILES independent tiles (a tile = 128 threads = 128 ray slots = one warpgroup). The tiles share the 20 KB
 // weight image — four separate CTAs would hold four copies — which matters because shared memory is carved out of the same
-// 256 KB as the L1 that serves the hash-grid gathers: 4 x 43.6 KB CTAs leave ~60 KB of L1, one 4-tile CTA (112 KB) leaves ~124 KB
-// (profiles/README.md: the tile loop runs 44 % faster with 92 KB of L1 than with 28 KB).
-// How many: as many as the register file allows without spilling. Frames without operators need 80 registers per thread -> 6 tiles (24 warps per SM,
-// 158 KB of shared memory, ~97 KB of L1): 10.96 ms per 1080p frame against 12.63 ms with 4 tiles and 11.51 ms with 5 (round 2, profiles/README.md
-// item 23; round 1's fatter loop spilled beyond 4). Frames with operators carry the deform / membrane state: 5 tiles (96 registers, 40 B spilled).
+// 256 KB as the L1 that serves the hash-grid gathers.
+// How many: the register file's worth. Frames without operators: 6 tiles (24 warps per SM, 80 registers per thread, 155 KB of shared memory);
+// the default fp16-accumulator build does not spill, the fp32 one spills 72 B per thread. Frames with operators carry the deform / membrane
+// state: 5 tiles (96 registers; 124-148 B spilled per thread with the wgmma layer chain). Other tile counts are not measured on the H100.
 #ifndef NSB_TILES
 #define NSB_TILES 6
 #endif
@@ -185,24 +183,20 @@ struct TileBlock {
 		uint8_t a32[tc::A32_BYTES];
 	};
 	float ray[R_FIELDS][128];
-	uint64_t mma_bar;
-	uint64_t pad[15];
 };
 template <int TILES>
 struct __align__(128) RenderSmemT {
 	uint8_t w[tc::W_BYTES];
 	TileBlock tile[TILES];
 	uint64_t w_bar;
-	uint32_t tmem_base;
-	uint32_t pad;
+	uint32_t pad[2];
 };
 __host__ __device__ constexpr int render_tiles(bool ops) { return ops ? NSB_TILES_OPS : NSB_TILES; }
-__host__ __device__ constexpr uint32_t render_tmem_cols(int tiles) { return tiles <= 1 ? 64u : tiles <= 2 ? 128u : tiles <= 4 ? 256u : 512u; }
-static_assert(NSB_TILES >= 1 && NSB_TILES <= 8 && NSB_TILES_OPS >= 1 && NSB_TILES_OPS <= 8, "64 TMEM columns per tile, 512 per SM");
+static_assert(NSB_TILES >= 1 && NSB_TILES <= 8 && NSB_TILES_OPS >= 1 && NSB_TILES_OPS <= 8, "1..8 tiles (warpgroups) per CTA");
 
 // OPS = false: the instantiation for frames without edit operators (f.apply_ops == 0 or no operator uploaded) carries none of the deform /
-// membrane code in its hot loop (the loop has to fit the instruction cache: profiles/README.md item 6).
-// ACC16: the MLP accumulator policy (nsb_set_mlp_accumulator): fp16 TMEM accumulators, like the reference's wmma __half fragments.
+// membrane code in its hot loop (the loop has to fit the instruction cache).
+// ACC16: the MLP accumulator policy (nsb_set_mlp_accumulator): fp16 wgmma accumulators, like the reference's wmma __half fragments.
 // experiment switches (tools/ab_kernels.py variants): compile a feature of the fused kernel out to measure what its presence costs the default path
 #ifndef NSB_X_ACCEL
 #define NSB_X_ACCEL 1
@@ -214,8 +208,7 @@ static_assert(NSB_TILES >= 1 && NSB_TILES <= 8 && NSB_TILES_OPS >= 1 && NSB_TILE
 #define NSB_X_RAYOD 1
 #endif
 #ifndef NSB_X_HELP
-#define NSB_X_HELP 0  // helper lanes: measured slower when used AND 5 % slower by their mere presence in the loop (register allocation / code layout):
-                      // compiled out of the product; `build.build_variant("helpers", ["NSB_X_HELP=1"])` is the experiment build NSB_HELPERS acts on
+#define NSB_X_HELP 0  // helper lanes: an experiment, compiled out of the product (their presence alone changes register allocation / code layout); `build.build_variant("helpers", ["NSB_X_HELP=1"])` is the experiment build NSB_HELPERS acts on
 #endif
 template <bool OPS, bool ACC16>
 __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(const DevFrame f, const DevModel m, const uint8_t* __restrict__ bitfield,
@@ -225,7 +218,6 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
                                                       unsigned long long* __restrict__ stats, const int refill_thr, const int dda_flags) {
 	extern __shared__ __align__(128) uint8_t smem_raw[];
 	constexpr int TILES = render_tiles(OPS);
-	constexpr uint32_t RENDER_TMEM_COLS = render_tmem_cols(TILES);
 	using RenderSmem = RenderSmemT<TILES>;
 	RenderSmem& RS = *reinterpret_cast<RenderSmem*>(smem_raw);
 	const uint32_t tid = threadIdx.x & 127u;      // slot / row within the tile
@@ -235,27 +227,12 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 	const uint32_t n_queued = *n_queued_ptr;
 	if (blockIdx.x * 128u * TILES >= n_queued && blockIdx.x > 0) return;  // nothing this CTA could ever fetch
 
-	// CTA setup: barriers, TMEM (64 columns per tile), one bulk-TMA copy of the weight image
-	if (threadIdx.x == 0) {
-		tc::mbar_init(&RS.w_bar, 1);
-		for (int t = 0; t < TILES; ++t) tc::mbar_init(&RS.tile[t].mma_bar, 1);
-		tc::fence_mbar_init();
-	}
-	if (threadIdx.x < 32) tc::tmem_alloc(&RS.tmem_base, RENDER_TMEM_COLS);
-	tc::tc_fence_before();
+	// CTA setup: one bulk-TMA copy of the weight image
+	tc::load_weights(RS.w, &RS.w_bar, m.w_image);
 	__syncthreads();
-	tc::tc_fence_after();
-	if (threadIdx.x < 32) {
-		if (threadIdx.x == 0) {
-			tc::mbar_expect_tx(&RS.w_bar, tc::W_BYTES);
-			tc::bulk_g2s(RS.w, m.w_image, tc::W_BYTES, &RS.w_bar);
-		}
-		__syncwarp();
-	}
 	tc::mbar_wait(&RS.w_bar, 0);
-	const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(&RS.tmem_base);
 	tc::TileCtx C;
-	C.a32 = TB.a32; C.a64 = TB.a64; C.w_addr = tc::smem_u32(RS.w); C.mma_bar = &TB.mma_bar; C.tmem = tmem_base + tile * tc::TMEM_COLS; C.row = tid;
+	C.a32 = TB.a32; C.w_addr = tc::smem_u32(RS.w); C.row = tid;
 	C.bar_id = 1 + tile;
 
 	const int dda_budget = dda_flags & 0xffff;
@@ -265,15 +242,14 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 	// encode and the MLPs. The owner lane then composites its own sample and, in march order, the helpers' — up to the first one that was not an
 	// occupied in-bounds sample, where the ordinary march resumes next round. Samples past a ray's termination are evaluated and discarded, like the
 	// reference's own n_steps > 1 batching; frames are bit-identical with or without helpers. help_mode 1: only once the queue is exhausted, 2: always.
-	// MEASURED (profiles/README.md, round 2): 13.5 % fewer rounds but each round 27 % dearer — the loop's cost follows the samples evaluated (gather
-	// wavefronts + issue), not the rounds — and the code's presence alone costs 5 %: it is compiled only into the experiment build (NSB_X_HELP=1).
+	// Compiled only into the experiment build (NSB_X_HELP=1); not measured on the H100.
 	const bool fx_show_accel = NSB_X_ACCEL && f.show_accel;
 	const int fx_glow = NSB_X_GLOW ? f.glow_mode : 0;
 	const float* const fx_ray_od = NSB_X_RAYOD ? ray_od : nullptr;
 	const int help_mode = (!NSB_X_HELP || OPS || (fx_glow & 4)) ? 0 : (dda_flags >> 16) & 3;  // host: NSB_HELPERS (the mailbox does not carry glow's weight mask)
 	constexpr uint32_t HELP_DEPTH = 7;
-	// mailbox helper -> owner: the tile's A-operand buffer is idle between the last MMA of a round and the next encode, and every warp only ever
-	// writes its own 32 rows of it: field q of lane l lives in k-chunk q, at this warp's 512 bytes
+	// mailbox helper -> owner: the tile's operand space is idle between the end of run_network (which ends on a tile barrier) and the next
+	// encode, and every warp only ever writes its own 512 bytes of each k-chunk: field q of lane l lives in k-chunk q
 	float* const mbox = reinterpret_cast<float*>(TB.a64 + (tid >> 5) * 512u) + lane;
 	constexpr uint32_t MB = tc::ROWS * 16 / 4;  // floats between mailbox fields
 	enum { M_ALPHA = 0, M_E0, M_E1, M_E2, M_Z, M_TNEXT };  // M_TNEXT < 0: not a sample
@@ -284,7 +260,6 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 	uint32_t ch_next = 0, ch_end = 0;       // this warp's chunk of the ray queue (warp-uniform)
 	uint32_t pix = 0, n_steps = 0;
 	uint32_t c_hit = 0, c_samples = 0, c_old = 0;
-	uint32_t phase = 0;
 	// phase profile (thread 0 of each CTA; a handful of clock reads per round): diagnostic builds only (-DNSB_PROFILE), the
 	// product build keeps the registers and issue slots (nsb_debug_counters then reports rounds and CTAs only)
 #ifdef NSB_PROFILE
@@ -478,7 +453,7 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 #ifdef NSB_PROFILE
 			enc_cycles += clock64() - e0;
 #endif
-			tc::run_network<ACC16>(C, phase, dw, old_pass, dens, rgbo);
+			tc::run_network<ACC16>(C, dw, old_pass, dens, rgbo);
 			if (old_pass) {
 				sigma_old_raw = h_lo(dens[0]);
 				if (need_old) ++c_old;
@@ -629,9 +604,6 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 		++n_rounds;
 	}
 
-	tc::tc_fence_before();
-	__syncthreads();  // all tiles done
-	if (threadIdx.x < 32) tc::tmem_dealloc(tmem_base, RENDER_TMEM_COLS);
 	if (tid == 0) {
 		atomicAdd(stats + ST_ROUNDS, (unsigned long long)n_rounds);
 #ifdef NSB_PROFILE
@@ -667,8 +639,7 @@ __global__ void __launch_bounds__(128) k_inference(const DevModel m, const float
 	extern __shared__ __align__(128) uint8_t smem_raw[];
 	tc::TileSmem& S = *reinterpret_cast<tc::TileSmem*>(smem_raw);
 	const uint32_t tid = threadIdx.x;
-	const uint32_t tmem_base = tc::tile_setup(S, m.w_image);
-	uint32_t phase = 0;
+	tc::tile_setup(S, m.w_image);
 	for (uint32_t base = blockIdx.x * 128u; base < n_padded; base += gridDim.x * 128u) {
 		uint32_t i = base + tid;
 		bool valid = i < n;
@@ -679,7 +650,7 @@ __global__ void __launch_bounds__(128) k_inference(const DevModel m, const float
 		}
 		uint32_t dens[8], rgbo[8];
 		encode_to_a32(S.a32, m, valid, pw, tid);
-		tc::run_network<ACC16>(tc::single_tile_ctx(S, tmem_base), phase, dw, DENSITY_ONLY, dens, rgbo);
+		tc::run_network<ACC16>(tc::single_tile_ctx(S), dw, DENSITY_ONLY, dens, rgbo);
 		if (i < n_padded) {
 			const uint32_t* src = DENSITY_ONLY ? dens : rgbo;
 #pragma unroll
@@ -690,7 +661,6 @@ __global__ void __launch_bounds__(128) k_inference(const DevModel m, const float
 			if (!DENSITY_ONLY) out[(size_t)3 * n_padded + i] = __ushort_as_half((unsigned short)(dens[0] & 0xffffu));  // extract_density
 		}
 	}
-	tc::tile_teardown(S, tmem_base);
 }
 
 // tcnn GridEncoding inference alone: fp16 [32 x n_padded] row-major, same loop body as the fused kernel.
@@ -859,9 +829,9 @@ __global__ void k_bitfield_max_pool(uint32_t n, const uint8_t* __restrict__ prev
 
 // ---- occupancy update through the edit operators (testbed_nerf.cu:3533-3639) ------------------------------------------
 // One fused pass per grid sample: draw (common_nerf.cu:179-208) -> map_positions in reverse operator order (:3593-3599)
-// -> hash encode + density MLP on tcgen05 (NerfNetwork::density) -> activate (:3522-3531) -> membrane residual density
+// -> hash encode + density MLP on wgmma (NerfNetwork::density) -> activate (:3522-3531) -> membrane residual density
 // (cage_deformation.cu:341-383) -> max-splat (:447-463). The reference materialises positions, indices, a bool mask and the
-// 16 x N fp16 density matrix between seven launches; here a sample lives in registers/shared memory/TMEM from draw to splat.
+// 16 x N fp16 density matrix between seven launches; here a sample lives in registers and shared memory from draw to splat.
 struct GridUpdateArgs {
 	uint32_t n_uniform, n_total, n_cascades, step;
 	uint64_t rng_state, rng_inc;
@@ -874,8 +844,7 @@ __global__ void __launch_bounds__(128) k_density_grid_update(const DevModel m, c
 	extern __shared__ __align__(128) uint8_t smem_raw[];
 	tc::TileSmem& S = *reinterpret_cast<tc::TileSmem*>(smem_raw);
 	const uint32_t tid = threadIdx.x;
-	const uint32_t tmem_base = tc::tile_setup(S, m.w_image);
-	uint32_t phase = 0;
+	tc::tile_setup(S, m.w_image);
 	const uint32_t n_padded = ((a.n_total + 127u) / 128u) * 128u;
 	for (uint32_t base = blockIdx.x * 128u; base < n_padded; base += gridDim.x * 128u) {
 		const uint32_t i = base + tid;
@@ -919,7 +888,7 @@ __global__ void __launch_bounds__(128) k_density_grid_update(const DevModel m, c
 		}
 		uint32_t dens[8], rgbo[8];
 		encode_to_a32(S.a32, m, valid, pw, tid);
-		tc::run_network<ACC16>(tc::single_tile_ctx(S, tmem_base), phase, dw, true, dens, rgbo);
+		tc::run_network<ACC16>(tc::single_tile_ctx(S), dw, true, dens, rgbo);
 		if (valid) {
 			__half h = __float2half_rn(network_to_density(__half2float(__ushort_as_half((unsigned short)(dens[0] & 0xffffu))), a.density_activation));
 			if (a.apply_ops) {
@@ -940,7 +909,6 @@ __global__ void __launch_bounds__(128) k_density_grid_update(const DevModel m, c
 			atomicMax(reinterpret_cast<unsigned int*>(grid_tmp) + idx, __float_as_uint(optical_thickness));  // uint order == float order for >= 0
 		}
 	}
-	tc::tile_teardown(S, tmem_base);
 }
 __global__ void k_ema_grid(uint32_t n, float decay, float* __restrict__ grid, const float* __restrict__ grid_tmp) {  // :483-506
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1125,9 +1093,9 @@ struct NsbContext {
 	size_t list_capacity = 0;
 	float* d_ray_od = nullptr;     // origin + direction per queue slot, general-camera frames only (allocated on the first such frame)
 	size_t ray_od_capacity = 0;
-	int acc16 = 1;                 // MLP accumulator policy: 1 fp16 TMEM accumulators (default: the reference's wmma __half fragments), 0 fp32 (nsb_set_mlp_accumulator)
+	int acc16 = 1;                 // MLP accumulator policy: 1 fp16 wgmma accumulators (default: the reference's wmma __half fragments), 0 fp32 (nsb_set_mlp_accumulator)
 	int use_ws = 0;                // NSB_WS=1: frames without operators go through the warp-specialised kernel (experimental; default k_render_fused<false>)
-	int helpers = 0;               // helper lanes of k_render_fused (experiment build only, -DNSB_X_HELP=1; measured slower: profiles/README.md): 0 off (default), 1 once the queue is exhausted, 2 always (NSB_HELPERS)
+	int helpers = 0;               // helper lanes of k_render_fused (experiment build only, -DNSB_X_HELP=1): 0 off (default), 1 once the queue is exhausted, 2 always (NSB_HELPERS)
 	int refill_thr = 2;            // lanes of a warp refill when at most this many of its rays are alive (31: immediately)
 	int dda_budget = DDA_BUDGET;
 	cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr;  // start, end, between k_prepare_rays and k_render_fused
@@ -1197,7 +1165,7 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 	CU(cudaSetDevice(device));
 	cudaDeviceProp prop;
 	CU(cudaGetDeviceProperties(&prop, device));
-	if (prop.major != 10) return fail(NSB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major, prop.minor);
+	if (prop.major != 9 || prop.minor != 0) return fail(NSB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
 	NsbContext* c = new NsbContext();
 	c->device = device;
 	c->sm_count = prop.multiProcessorCount;
@@ -1215,7 +1183,7 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 	}
 	// Shared memory and L1 share one 256 KB array per SM: every kernel asks for exactly the carve-out its resident CTAs need and
 	// leaves the rest to L1, which serves the hash-grid gathers (the default heuristic picks a carve-out too small for even one
-	// CTA; "max shared" starves L1 — the tile loop runs 44 % faster with 92 KB of L1 than with 28 KB, profiles/README.md).
+	// CTA; "max shared" starves L1).
 	auto set_smem = [&](const void* func, size_t bytes_per_cta, int ctas) -> cudaError_t {
 		cudaError_t e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes_per_cta);
 		if (e != cudaSuccess) return e;
@@ -1224,8 +1192,8 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 		if (pct > 100) pct = 100;
 		return cudaFuncSetAttribute(func, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
 	};
-	// k_render_fused: ONE CTA of NSB_TILES (NSB_TILES_OPS with operators) tiles per SM (768 x 80 / 640 x 96 registers = the register file; TMEM 64 columns
-	// per tile; shared memory 20 KB weights + 23 KB per tile).
+	// k_render_fused: ONE CTA of NSB_TILES (NSB_TILES_OPS with operators) tiles per SM (768 x 80 / 640 x 96 registers = the register file;
+	// shared memory 20 KB weights + 22.5 KB per tile).
 	c->ctas_per_sm = 1;
 	CU(set_smem((const void*)k_render_fused<false, false>, sizeof(RenderSmemT<render_tiles(false)>), 1));
 	CU(set_smem((const void*)k_render_fused<true, false>, sizeof(RenderSmemT<render_tiles(true)>), 1));
@@ -1308,7 +1276,7 @@ extern "C" NsbStatus nsb_destroy(NsbContext* c) {
 	return NSB_OK;
 }
 
-// [N x K] row-major fp16 -> UMMA K-major no-swizzle operand image (nsb_tc.cuh header comment)
+// [N x K] row-major fp16 -> wgmma K-major no-swizzle operand image (nsb_tc.cuh header comment)
 static void to_operand_layout(const uint16_t* W, uint32_t N, uint32_t K, uint8_t* dst) {
 	for (uint32_t n = 0; n < N; ++n)
 		for (uint32_t k = 0; k < K; ++k) {
@@ -1317,7 +1285,7 @@ static void to_operand_layout(const uint16_t* W, uint32_t N, uint32_t K, uint8_t
 		}
 }
 
-// params_on_device: the block is read where tcnn::Trainer keeps it; only the 20 KB of MLP weights pass through the host (to be laid out as UMMA operands)
+// params_on_device: the block is read where tcnn::Trainer keeps it; only the 20 KB of MLP weights pass through the host (to be laid out as wgmma operands)
 static NsbStatus upload_model_impl(NsbContext* c, const NsbModelDesc* desc, const uint16_t* params, uint64_t n_params, bool params_on_device) {
 	if (!c || !desc || !params) return fail(NSB_ERR_INVALID, "null argument");
 	CU(cudaSetDevice(c->device));

@@ -1,14 +1,13 @@
 // nsb_render_ws.cuh — the warp-specialised form of the fused persistent renderer (frames without edit operators).
 //
-// k_render_fused lets every warp do everything: march -> 128 gathers -> five MMA layers (six tile-wide barriers) -> composite, serially,
-// per round. Its profile (profiles/README.md, round 2) is issue-/latency-bound at 16 warps per SM with ~30 % of the stall samples on the tile
-// barriers and the MMA completion waits. Here the two halves of a round run concurrently on different warps of ONE 768-thread CTA per SM:
+// k_render_fused lets every warp do everything: march -> 128 gathers -> five MMA layers (tile-wide barriers) -> composite, serially,
+// per round. Here the two halves of a round run concurrently on different warps of ONE 768-thread CTA per SM (an experiment, opt-in NSB_WS=1):
 //
 //   producers (16 warps = 4 tiles x 128 ray slots): own the rays' march state. Per generation: learn which of their rays the consumers
 //       terminated, refill free slots (same warp-coherent policy as the fused kernel), walk the occupancy grid to the next sample, gather the
-//       32 hash-grid features straight into a double-buffered UMMA A operand in shared memory, publish {t, flags, pixel} and arrive on the
+//       32 hash-grid features straight into the first layer's wgmma A operand in shared memory, publish {t, flags, pixel} and arrive on the
 //       tile's `full` mbarrier. They never wait for a tile barrier or an MMA.
-//   consumers (8 warps = 2 groups x 128 rows, each group serves two producer tiles alternately): wait for `full`, run the five tcgen05
+//   consumers (8 warps = 2 warpgroups x 128 rows, each group serves two producer tiles alternately): wait for `full`, run the five wgmma
 //       layers (first layer reads the producers' operand in place), composite the sample into the ray's accumulators, shade finished rays,
 //       record terminations, and arrive on `empty`.
 //
@@ -29,15 +28,14 @@ constexpr int PT = NSB_WS_PT;         // producer tiles (128 ray slots each)
 constexpr int CG = NSB_WS_CG;         // consumer groups (128 threads each)
 constexpr int TPG = PT / CG;          // producer tiles per consumer group
 constexpr int THREADS = (PT + CG) * 128;
-constexpr uint32_t TMEM_COLS_TOTAL = CG * TPG * 64 <= 64 ? 64 : CG * TPG * 64 <= 128 ? 128 : CG * TPG * 64 <= 256 ? 256 : 512;  // 64 accumulator columns per producer tile
-static_assert(PT == 2 * CG, "a consumer group walks the layer chain for TWO producer tiles at once");
+static_assert(PT == 2 * CG, "a consumer group serves TWO producer tiles");
 
 enum { F_SAMPLE = 1u, F_FIRST = 2u, F_EXIT = 4u, F_DROP = 8u };
 enum { S_PX = 0, S_PY, S_PZ, S_DT, S_DX, S_DY, S_DZ, S_FLAGS, S_FIELDS };  // per sample: warped position, warped dt, warped direction, flags (F_FIRST: S_DT holds the pixel)
 // consumer-side ray state, parked in shared memory between generations (a group alternates between two tiles)
 enum { A_CR = 0, A_CG, A_CB, A_CA, A_DEPTH, A_MAXW, A_PIX, A_META, A_FIELDS };  // META: bit 31 alive, low bits n_steps
 
-struct __align__(128) Tile {  // the UMMA descriptors address feat in 16-byte units
+struct __align__(128) Tile {  // the wgmma descriptors address feat in 16-byte units
 	uint8_t feat[tc::A32_BYTES];           // ONE operand buffer: released (feat_free) as soon as the first layer's MMAs have completed, long before the generation is done
 	uint32_t out[3][128];                  // network outputs the composite needs: density raw | (r, g) | (b, -) as packed fp16
 	uint64_t feat_free;
@@ -50,17 +48,14 @@ struct __align__(128) Tile {  // the UMMA descriptors address feat in 16-byte un
 	uint32_t cepoch[128];  // consumer's ray counter per slot
 };
 struct __align__(128) Group {
-	uint8_t a64[TPG][tc::A64_BYTES];
-	uint64_t mma_bar;
-	uint64_t pad[15];
+	uint8_t a64[tc::A64_BYTES];  // the group's operand space (rgb-network input, output hand-back)
 };
 struct __align__(128) Smem {
 	uint8_t w[tc::W_BYTES];
 	Tile tile[PT];
 	Group grp[CG];
 	uint64_t w_bar;
-	uint32_t tmem_base;
-	uint32_t pad;
+	uint32_t pad[2];
 };
 
 }  // namespace ws
@@ -76,13 +71,11 @@ __global__ void __launch_bounds__(ws::THREADS, 1) k_render_ws(const DevFrame f, 
 	if (blockIdx.x * 128u * PT >= n_queued && blockIdx.x > 0) return;  // nothing this CTA could ever fetch
 
 	if (threadIdx.x == 0) {
-		tc::mbar_init(&S.w_bar, 1);
 		for (int t = 0; t < PT; ++t) {
 			for (int b = 0; b < 2; ++b) { tc::mbar_init(&S.tile[t].full[b], 4); tc::mbar_init(&S.tile[t].empty[b], 4); }
 			tc::mbar_init(&S.tile[t].feat_free, 1);
 			S.tile[t].stop = 0;
 		}
-		for (int g = 0; g < CG; ++g) tc::mbar_init(&S.grp[g].mma_bar, 1);
 		tc::fence_mbar_init();
 	}
 	for (uint32_t i = threadIdx.x; i < PT * 128u; i += THREADS) {
@@ -90,18 +83,8 @@ __global__ void __launch_bounds__(ws::THREADS, 1) k_render_ws(const DevFrame f, 
 		S.tile[i >> 7].cepoch[i & 127u] = 0u;
 		S.tile[i >> 7].acc[A_META][i & 127u] = __uint_as_float(0u);
 	}
-	if (warp == 0) tc::tmem_alloc(&S.tmem_base, TMEM_COLS_TOTAL);
-	tc::tc_fence_before();
+	tc::load_weights(S.w, &S.w_bar, m.w_image);
 	__syncthreads();
-	tc::tc_fence_after();
-	if (warp == 0) {
-		if (lane == 0) {
-			tc::mbar_expect_tx(&S.w_bar, tc::W_BYTES);
-			tc::bulk_g2s(S.w, m.w_image, tc::W_BYTES, &S.w_bar);
-		}
-		__syncwarp();
-	}
-	const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(&S.tmem_base);
 
 	uint32_t c_hit = 0, c_samples = 0, n_gen = 0;
 #ifdef NSB_PROFILE
@@ -216,50 +199,17 @@ __global__ void __launch_bounds__(ws::THREADS, 1) k_render_ws(const DevFrame f, 
 #endif
 	} else {
 		// =============================================== consumer ===============================================
-		// A group walks the five layers for its TWO producer tiles together: per layer one tile barrier, both tiles' MMAs issued back to back
-		// with one completion wait, then both epilogues — half the barriers and waits per sample of the one-tile chain.
+		// A group (one warpgroup) runs the network for its two producer tiles one after the other; the first layer reads the producer's operand
+		// in place and releases it (feat_free) as soon as every warp of the group has read it.
 		const uint32_t grp = warp >> 2, row = threadIdx.x & 127u;
 		Group& G = S.grp[grp];
 		Tile& TA = S.tile[grp * TPG + 0];
 		Tile& TB = S.tile[grp * TPG + 1];
 		tc::mbar_wait(&S.w_bar, 0);
-		const uint32_t w_addr = tc::smem_u32(S.w);
-		const uint32_t tmemA = tmem_base + (grp * TPG + 0) * tc::TMEM_COLS, tmemB = tmem_base + (grp * TPG + 1) * tc::TMEM_COLS;
-		const uint32_t lane_field = (row & ~31u) << 16;
-		const uint32_t a64A = tc::smem_u32(G.a64[0]), a64B = tc::smem_u32(G.a64[1]);
-		const uint32_t featA = tc::smem_u32(TA.feat), featB = tc::smem_u32(TB.feat);
-		const uint32_t bar_id = 1 + grp;
-		uint32_t phase = 0;
+		tc::TileCtx C;
+		C.a32 = G.a64; C.w_addr = tc::smem_u32(S.w); C.row = row; C.bar_id = 1 + grp;
 		const float sat = 1.0f - f.min_T;
 		const V3 cam_fwd = v3(f.cam1[6], f.cam1[7], f.cam1[8]);
-		// one layer for both tiles: D_A = A_A W^T, D_B = A_B W^T; `release` = also arrive on the tiles' feat_free barriers (first layer)
-		auto layer = [&](auto n_tag, auto k_tag, uint32_t aA, uint32_t aB, uint32_t w_off, bool release) {
-			constexpr uint32_t N = decltype(n_tag)::value, K = decltype(k_tag)::value;
-			tc::fence_async_smem();
-			tc::tc_fence_before();
-			asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-			if (row < 32) {
-				if (row == 0) {
-					tc::tc_fence_after();
-					constexpr uint32_t idesc = tc::make_idesc(tc::ROWS, N);
-#pragma unroll
-					for (uint32_t k = 0; k < K / 16; ++k)
-						tc::umma_f16(tmemA, tc::make_desc(aA + k * 2 * (tc::ROWS * 16), tc::ROWS * 16, 128), tc::make_desc(w_addr + w_off + k * 2 * (N * 16), N * 16, 128), idesc, k > 0 ? 1u : 0u);
-#pragma unroll
-					for (uint32_t k = 0; k < K / 16; ++k)
-						tc::umma_f16(tmemB, tc::make_desc(aB + k * 2 * (tc::ROWS * 16), tc::ROWS * 16, 128), tc::make_desc(w_addr + w_off + k * 2 * (N * 16), N * 16, 128), idesc, k > 0 ? 1u : 0u);
-					tc::umma_commit(&G.mma_bar);
-				}
-				__syncwarp();
-			}
-			tc::mbar_wait(&G.mma_bar, phase);
-			phase ^= 1;
-			tc::tc_fence_after();
-			if (release && row == 0) { tc::mbar_arrive(&TA.feat_free); tc::mbar_arrive(&TB.feat_free); }  // the MMAs have read the producers' operands
-		};
-		using I16 = std::integral_constant<uint32_t, 16>;
-		using I32 = std::integral_constant<uint32_t, 32>;
-		using I64 = std::integral_constant<uint32_t, 64>;
 		for (uint32_t g = 0;; ++g) {
 			const uint32_t b = g & 1u;
 #ifdef NSB_PROFILE
@@ -285,47 +235,17 @@ __global__ void __launch_bounds__(ws::THREADS, 1) k_render_ws(const DevFrame f, 
 				}
 			}
 			if (row == 0) ++n_gen;
-			// ---- the five layers, both tiles ----
-			layer(I64{}, I32{}, featA, featB, tc::W1_OFF, true);
-			tc::epilogue_hidden(G.a64[0], tmemA + lane_field, row);
-			tc::epilogue_hidden(G.a64[1], tmemB + lane_field, row);
-			layer(I16{}, I64{}, a64A, a64B, tc::W2_OFF, false);
-#pragma unroll
-			for (int k = 0; k < 2; ++k) {  // density MLP output (16) + SH(direction) (16) = the rgb network's input, in place
-				Tile& TL = k ? TB : TA;
-				uint32_t r[16];
-				tc::tmem_ld16((k ? tmemB : tmemA) + lane_field, r);
-				tc::tmem_wait_ld();
-				uint32_t d[8];
-#pragma unroll
-				for (int i = 0; i < 8; ++i) d[i] = tc::pack(r[2 * i], r[2 * i + 1]);
-				TL.out[0][row] = d[0];
+			// ---- the five layers, one tile after the other ----
+#pragma unroll 1
+			for (uint32_t k = 0; k < (uint32_t)TPG; ++k) {
+				Tile& TL = S.tile[grp * TPG + k];
 				const V3 dw = v3(__uint_as_float(TL.side[b][S_DX][row]), __uint_as_float(TL.side[b][S_DY][row]), __uint_as_float(TL.side[b][S_DZ][row]));
-				__half2 sh[8];
-				encode_sh4(dw, sh);
-				uint8_t* a32 = G.a64[k];
-				tc::store_chunk(a32, 0, row, make_uint4(d[0], d[1], d[2], d[3]));
-				tc::store_chunk(a32, 1, row, make_uint4(d[4], d[5], d[6], d[7]));
-				tc::store_chunk(a32, 2, row, make_uint4(tc::pack_h2(sh[0]), tc::pack_h2(sh[1]), tc::pack_h2(sh[2]), tc::pack_h2(sh[3])));
-				tc::store_chunk(a32, 3, row, make_uint4(tc::pack_h2(sh[4]), tc::pack_h2(sh[5]), tc::pack_h2(sh[6]), tc::pack_h2(sh[7])));
+				uint32_t dens[8], rgbo[8];
+				tc::run_network<false>(C, dw, false, dens, rgbo, tc::smem_u32(TL.feat), &TL.feat_free);
+				TL.out[0][row] = dens[0];
+				TL.out[1][row] = rgbo[0];
+				TL.out[2][row] = rgbo[1];
 			}
-			layer(I64{}, I32{}, a64A, a64B, tc::W3_OFF, false);
-			tc::epilogue_hidden(G.a64[0], tmemA + lane_field, row);
-			tc::epilogue_hidden(G.a64[1], tmemB + lane_field, row);
-			layer(I64{}, I64{}, a64A, a64B, tc::W4_OFF, false);
-			tc::epilogue_hidden(G.a64[0], tmemA + lane_field, row);
-			tc::epilogue_hidden(G.a64[1], tmemB + lane_field, row);
-			layer(I16{}, I64{}, a64A, a64B, tc::W5_OFF, false);
-#pragma unroll
-			for (int k = 0; k < 2; ++k) {
-				uint32_t r[4];
-				tc::tmem_ld4((k ? tmemB : tmemA) + lane_field, r);
-				tc::tmem_wait_ld();
-				Tile& TL = k ? TB : TA;
-				TL.out[1][row] = tc::pack(r[0], r[1]);
-				TL.out[2][row] = tc::pack(r[2], r[3]);
-			}
-			tc::tc_fence_before();
 			// ---- composite (composite_kernel_nerf :750-955) + shade (shade_kernel_nerf :2464-2482), one tile after the other ----
 #pragma unroll 1
 			for (uint32_t k = 0; k < (uint32_t)TPG; ++k) {
@@ -424,9 +344,6 @@ __global__ void __launch_bounds__(ws::THREADS, 1) k_render_ws(const DevFrame f, 
 #endif
 	}
 
-	tc::tc_fence_before();
-	__syncthreads();
-	if (warp == 0) tc::tmem_dealloc(tmem_base, ws::TMEM_COLS_TOTAL);
 	if (threadIdx.x == 0) {
 		atomicAdd(stats + ST_ROUNDS, (unsigned long long)n_gen);
 		atomicAdd(stats + ST_CTAS, 1ull);

@@ -1,19 +1,21 @@
-// nsb_tc.cuh — 5th-gen tensor core (tcgen05 / TMEM) plumbing for the fully fused 64-wide MLPs.
+// nsb_tc.cuh — Hopper warpgroup tensor core (wgmma) plumbing for the fully fused 64-wide MLPs.
 //
-// Geometry: one CTA = 128 threads = 128 samples = the M dimension of every UMMA (M=128), thread t owns
-// sample row t, TMEM lane t, and (in the fused renderer) ray t. The five layers
+// Geometry: one tile = 128 threads = one warpgroup = 128 samples; thread t owns sample t and (in the fused renderer) ray t.
+// The five layers
 //     L1 32->64 (ReLU)  L2 64->16        (density MLP, base.json "network")
 //     L3 32->64 (ReLU)  L4 64->64 (ReLU)  L5 64->16   (rgb MLP, "rgb_network")
-// are 2+4+2+4+4 = 16 tcgen05.mma.kind::f16 instructions (K=16 each) with fp32 accumulators in TMEM.
-// Activations never leave the SM: encode/epilogue threads write fp16 rows straight into the UMMA
-// A-operand layout in shared memory, the weights (20 KB) are staged once per CTA by a bulk-TMA copy.
+// run as wgmma.mma_async m64nNk16 (K=16 per instruction), one M=64 half of the tile at a time, accumulators in registers.
+// L1 and L3 read their A operand from shared memory (written row by row by the threads that own the samples); L2, L4 and L5
+// take it straight from the previous layer's accumulators (the m64nNk16 accumulator fragment is the A fragment of the next
+// layer), so hidden activations never leave the registers. The weights (20 KB) are staged once per CTA by a bulk-TMA copy.
 //
-// Shared-memory operand layout (K-major, no swizzle = UMMA "interleave" canonical layout,
-// cute/atom/mma_traits_sm100.hpp: ((8,m),(T,2)):((1T,SBO),(1,LBO)) in 16-byte units):
-//   element (row r, k) of an [R x K] fp16 operand lives at  (k/8)*(R*16) + r*16 + (k%8)*2  bytes
+// Shared-memory operand layout (K-major, no swizzle = the wgmma "interleave" canonical layout
+// ((8,m),(T,2)):((1T,SBO),(1,LBO)) in 16-byte units):
+//   element (physical row p, k) of an [R x K] fp16 operand lives at  (k/8)*(R*16) + p*16 + (k%8)*2  bytes
 //   -> core matrix = 8 rows x 16 B contiguous (128 B); SBO (next 8 rows) = 128 B; LBO (next 8 k) = R*16 B.
-// A thread writing its own row touches 16 contiguous bytes per k-chunk, and the 32 lanes of a warp cover
-// 512 contiguous bytes: conflict-free stores without padding.
+// Row permutation: warp w of a warpgroup receives accumulator rows 16w..16w+15 of each M=64 half. Sample t is stored at physical
+// row phys_row(t) = 64*((t%32)/16) + 16*(t/32) + t%16, so every accumulator row a warp receives belongs to one of its own 32
+// threads: the result hand-back to the owning thread is a warp-local exchange through the warp's own operand rows.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -24,7 +26,7 @@
 namespace nsb {
 namespace tc {
 
-constexpr uint32_t ROWS = 128;                    // samples per tile = UMMA M
+constexpr uint32_t ROWS = 128;                    // samples per tile = one warpgroup, two M=64 halves
 constexpr uint32_t A32_BYTES = 4 * ROWS * 16;     // [4 k-chunks][128][16 B]
 constexpr uint32_t A64_BYTES = 8 * ROWS * 16;
 // weight image: W1 [64x32], W2 [16x64], W3 [64x32], W4 [64x64], W5 [16x64], each in the operand layout above
@@ -34,24 +36,21 @@ constexpr uint32_t W3_OFF = W2_OFF + 16 * 64 * 2;
 constexpr uint32_t W4_OFF = W3_OFF + 64 * 32 * 2;
 constexpr uint32_t W5_OFF = W4_OFF + 64 * 64 * 2;
 constexpr uint32_t W_BYTES = W5_OFF + 16 * 64 * 2;  // 20480
-constexpr uint32_t TMEM_COLS = 64;
 
-// The 32-wide operand (L1 / L3 input) aliases the first half of the 64-wide one (L2 / L4 / L5 input): at every point of
-// the layer chain only one of them is live (the MMA that read the other has completed before the epilogue overwrites it),
-// so a tile needs 16 KB of operand space, 36.9 KB with the weights.
+// Operand space of a tile: chunks 0-3 = the 32-wide layer input (grid features for L1; density output + SH for L3), chunks 4-5 =
+// the hand-back of the rgb output. The a32 view aliases the first half of a64.
 struct __align__(128) TileSmem {
 	uint8_t w[W_BYTES];
 	union {
 		uint8_t a64[A64_BYTES];
 		uint8_t a32[A32_BYTES];
 	};
-	uint64_t mma_bar;
 	uint64_t w_bar;
-	uint32_t tmem_base;
-	uint32_t pad;
+	uint32_t pad[2];
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__host__ __device__ __forceinline__ uint32_t phys_row(uint32_t t) { return ((t & 16u) << 2) | ((t >> 5) << 4) | (t & 15u); }
 
 // ---- mbarrier -----------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -64,7 +63,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-// Bounded wait: a broken pipeline traps (after ~2 s) instead of hanging the GPU box.
+// Bounded wait: a broken pipeline traps (after ~2 s) instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 	uint32_t addr = smem_u32(bar);
 	uint32_t done = 0;
@@ -116,101 +115,139 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 // generic-proxy shared stores -> visible to the async proxy (tensor core operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- TMEM ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t cols) {  // one full warp
-	asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols) : "memory");
-	asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {  // the allocating warp
-	asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32-bit, 16 consecutive columns: thread i of the warp gets lane (base_lane + i), columns c..c+15
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-	asm volatile(
-		"tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-		: "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-		  "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-		: "r"(taddr)
-		: "memory");
-}
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, uint32_t* r) {
-	asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-	             : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-	             : "r"(taddr)
-	             : "memory");
+// One thread stages the weight image (bulk TMA) and initialises the barrier; the caller's __syncthreads() publishes the init,
+// then every thread waits for the copy.
+__device__ __forceinline__ void load_weights(uint8_t* w, uint64_t* w_bar, const uint8_t* __restrict__ w_image) {
+	if (threadIdx.x == 0) {
+		mbar_init(w_bar, 1);
+		fence_mbar_init();
+		mbar_expect_tx(w_bar, W_BYTES);
+		bulk_g2s(w, w_image, W_BYTES, w_bar);
+	}
 }
 
-// ---- UMMA descriptors -----------------------------------------------------------------------------
-// cute::UMMA::SmemDescriptor (cute/arch/mma_sm100_desc.hpp): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
-// version=1 [46,48), base_offset [49,52)=0, lbo_mode [52]=0, layout_type [61,64)=0 (SWIZZLE_NONE).
+// ---- wgmma ------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (sm_90 GMMA): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), base_offset [49,52)=0,
+// layout_type [62,64)=0 (INTERLEAVE, no swizzle).
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
 	uint64_t d = 0;
 	d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);
 	d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
 	d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;
-	d |= (uint64_t)1 << 46;
 	return d;
 }
-// cute::UMMA::InstrDescriptor for kind::f16: D=F32 (c_format 1 @ [4,6)), A=B=F16 (0), both K-major (0),
-// N>>3 @ [17,23), M>>4 @ [24,29).
-// acc16: D=F16 (c_format 0) — the accumulator is rounded to fp16 by every K=16 instruction, the arithmetic of wmma m16n16k16 with __half
-// accumulator fragments (tiny-cuda-nn's FullyFusedMLP of the reference's era); each fp16 still occupies one 32-bit TMEM column (low half).
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t M, uint32_t N, bool acc16 = false) { return (acc16 ? 0u : (1u << 4)) | ((N >> 3) << 17) | ((M >> 4) << 24); }
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-	asm volatile(
-		"{\n\t.reg .pred p;\n\t"
-		"setp.ne.b32 p, %4, 0;\n\t"
-		"tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-		:
-		: "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-		: "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-	asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// One layer: D[128 x N] = A[128 x K] * W[N x K]^T, issued by ONE thread; completion arrives on mma_bar.
-template <uint32_t N, uint32_t K, bool ACC16 = false>
-__device__ __forceinline__ void issue_layer(uint32_t tmem_d, uint32_t a_addr, uint32_t w_addr, uint64_t* bar) {
-	constexpr uint32_t idesc = make_idesc(ROWS, N, ACC16);
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMA
+template <int NR> __device__ __forceinline__ void reg_fence(uint32_t* r) {
 #pragma unroll
-	for (uint32_t k = 0; k < K / 16; ++k) {
-		// one instruction consumes K=16 = two 8-wide k-chunks; chunk stride = rows*16 bytes
-		uint64_t ad = make_desc(a_addr + k * 2 * (ROWS * 16), ROWS * 16, 128);
-		uint64_t bd = make_desc(w_addr + k * 2 * (N * 16), N * 16, 128);
-		umma_f16(tmem_d, ad, bd, idesc, k > 0 ? 1u : 0u);
-	}
-	umma_commit(bar);
+	for (int i = 0; i < NR; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 
-// The MMA is issued by lane 0 of warp 0, but the WHOLE warp takes the branch and re-converges before anybody
-// waits on the mbarrier: if lanes 1-31 reached mbarrier.try_wait first (divergent from lane 0), the warp would
-// sleep in the hardware wait until its time-out before lane 0 ever issued the instruction it is waiting for.
-template <uint32_t N, uint32_t K, bool ACC16 = false>
-__device__ __forceinline__ void issue_converged(uint32_t row, uint32_t tmem_d, uint32_t a_addr, uint32_t w_addr, uint64_t* bar) {
-	if (row < 32) {  // warp 0 of the tile
-		if (row == 0) {
-			tc_fence_after();
-			issue_layer<N, K, ACC16>(tmem_d, a_addr, w_addr, bar);
-		}
-		__syncwarp();
-	}
+// Accumulators per thread of one m64nNk16: N/2 fp32 (ACC16 = false) or N/4 packed half2 (ACC16 = true), as 32-bit registers.
+// acc16: D=F16 — the accumulator is rounded to fp16 by every K=16 instruction, the arithmetic of wmma m16n16k16 with __half
+// accumulator fragments (tiny-cuda-nn's FullyFusedMLP of the reference's era).
+template <uint32_t N, bool ACC16> struct Acc { static constexpr int R = ACC16 ? (int)N / 4 : (int)N / 2; uint32_t r[R] = {}; };
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T. _ss: A from shared memory (descriptor); _rs: A from registers (4 x half2 fragment).
+// B is the weight operand in shared memory; scale_d = 0 overwrites D. Both operands K-major (no transpose).
+template <uint32_t N, bool ACC16> __device__ __forceinline__ void wgmma_ss(uint32_t* d, uint64_t ad, uint64_t bd, uint32_t scale_d);
+template <uint32_t N, bool ACC16> __device__ __forceinline__ void wgmma_rs(uint32_t* d, const uint32_t* a, uint64_t bd, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_ss<64, false>(uint32_t* d, uint64_t ad, uint64_t bd, uint32_t scale_d) {
+	asm volatile(
+		"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+		: "l"(ad), "l"(bd), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_ss<64, true>(uint32_t* d, uint64_t ad, uint64_t bd, uint32_t scale_d) {
+	asm volatile(
+		"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n64k16.f16.f16.f16 "
+		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+		: "l"(ad), "l"(bd), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_rs<64, false>(uint32_t* d, const uint32_t* a, uint64_t bd, uint32_t scale_d) {
+	asm volatile(
+		"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+		: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_rs<64, true>(uint32_t* d, const uint32_t* a, uint64_t bd, uint32_t scale_d) {
+	asm volatile(
+		"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n64k16.f16.f16.f16 "
+		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+		: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_rs<16, false>(uint32_t* d, const uint32_t* a, uint64_t bd, uint32_t scale_d) {
+	asm volatile(
+		"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+		"{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+		: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_rs<16, true>(uint32_t* d, const uint32_t* a, uint64_t bd, uint32_t scale_d) {
+	asm volatile(
+		"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %9, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n16k16.f16.f16.f16 "
+		"{%0, %1, %2, %3}, {%4, %5, %6, %7}, %8, p, 1, 1, 0;\n\t}"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+		: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
 }
 
-// ---- a tile = 128 threads (4 warps, TMEM lanes 0-127) walking the layer chain together. A CTA may hold several tiles
-// (they share the weight image; each has its own operands, mbarrier, TMEM columns and named barrier).
+// ---- fragments --------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t pack_h2(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
+__device__ __forceinline__ uint32_t pack(uint32_t a_bits, uint32_t b_bits) {
+	return pack_h2(__floats2half2_rn(__uint_as_float(a_bits), __uint_as_float(b_bits)));
+}
+// ReLU after the fp16 conversion: rounding is monotone and 0 is exact, so max(cvt(x), 0) == cvt(max(x, 0)) — one packed
+// HMNMX2 per pair instead of two FMNMX.
+__device__ __forceinline__ uint32_t relu_h2(uint32_t p) { return pack_h2(__hmax2(*reinterpret_cast<__half2*>(&p), __floats2half2_rn(0.0f, 0.0f))); }
+// Element pair i of an accumulator as packed half2, in fragment order: pair i covers row (lane/4 + 8*(i&1)), columns 8*(i/2) + 2*(lane%4) + {0,1}
+// of the warp's 16 rows. fp32 accumulators are rounded here, fp16 accumulators already are pairs.
+template <bool ACC16> __device__ __forceinline__ uint32_t acc_pair(const uint32_t* d, int i) { return ACC16 ? d[i] : pack(d[2 * i], d[2 * i + 1]); }
+
+// One layer on one M=64 half: D = A * W^T with A in shared memory (a_addr = the half's first row, k-chunk stride ROWS*16)
+template <uint32_t N, uint32_t K, bool ACC16>
+__device__ __forceinline__ void layer_ss(uint32_t* d, uint32_t a_addr, uint32_t w_addr) {
+	wg_fence();
+#pragma unroll
+	for (uint32_t k = 0; k < K / 16; ++k)  // one instruction consumes K=16 = two 8-wide k-chunks
+		wgmma_ss<N, ACC16>(d, make_desc(a_addr + k * 2 * (ROWS * 16), ROWS * 16, 128), make_desc(w_addr + k * 2 * (N * 16), N * 16, 128), k > 0 ? 1u : 0u);
+	wg_commit();
+	wg_wait();
+	reg_fence<Acc<N, ACC16>::R>(d);
+}
+// ... with A = ReLU(the previous layer's accumulators `x` of width K): the accumulator fragment of columns 16k..16k+15 is the A fragment of k-step k
+template <uint32_t N, uint32_t K, bool ACC16>
+__device__ __forceinline__ void layer_rs(uint32_t* d, const uint32_t* x, uint32_t w_addr) {
+	uint32_t a[K / 16][4];
+#pragma unroll
+	for (uint32_t k = 0; k < K / 16; ++k)
+#pragma unroll
+		for (int i = 0; i < 4; ++i) a[k][i] = relu_h2(acc_pair<ACC16>(x, 4 * (int)k + i));
+	wg_fence();
+#pragma unroll
+	for (uint32_t k = 0; k < K / 16; ++k) wgmma_rs<N, ACC16>(d, a[k], make_desc(w_addr + k * 2 * (N * 16), N * 16, 128), k > 0 ? 1u : 0u);
+	wg_commit();
+	wg_wait();
+	reg_fence<Acc<N, ACC16>::R>(d);
+}
+
+// ---- a tile = 128 threads (one warpgroup) walking the layer chain together. A CTA may hold several tiles
+// (they share the weight image; each has its own operand space and named barrier).
 struct TileCtx {
-	uint8_t* a32;        // 32-wide operand (aliases the first half of a64)
-	uint8_t* a64;
+	uint8_t* a32;        // operand space (A64_BYTES); the 32-wide operand is its first half
 	uint32_t w_addr;     // shared-window address of the weight image
-	uint64_t* mma_bar;
-	uint32_t tmem;       // TMEM address of this tile's column 0, lane 0
-	uint32_t row;        // 0..127 within the tile
+	uint32_t row;        // sample 0..127 within the tile
 	uint32_t bar_id;     // named barrier of the tile (0 = the CTA barrier when the CTA is one tile)
 };
 __device__ __forceinline__ void tile_sync(const TileCtx& c) { asm volatile("bar.sync %0, 128;" ::"r"(c.bar_id) : "memory"); }
@@ -227,134 +264,94 @@ __device__ __forceinline__ bool tile_any(const TileCtx& c, bool p) {
 	return r != 0;
 }
 
-// ---- tile lifecycle -------------------------------------------------------------------------------
-// All 128 threads call; returns the TMEM base address (lane 0, column 0 of this CTA's 64 columns).
-__device__ __forceinline__ uint32_t tile_setup(TileSmem& s, const uint8_t* __restrict__ w_image) {
-	const uint32_t tid = threadIdx.x;
-	if (tid == 0) {
-		mbar_init(&s.mma_bar, 1);
-		mbar_init(&s.w_bar, 1);
-		fence_mbar_init();
-	}
-	if (tid < 32) tmem_alloc(&s.tmem_base, TMEM_COLS);
-	tc_fence_before();
+// ---- tile lifecycle (one-tile CTAs) ----------------------------------------------------------------
+__device__ __forceinline__ void tile_setup(TileSmem& s, const uint8_t* __restrict__ w_image) {
+	load_weights(s.w, &s.w_bar, w_image);
 	__syncthreads();
-	tc_fence_after();
-	if (tid < 32) {
-		if (tid == 0) {
-			mbar_expect_tx(&s.w_bar, W_BYTES);
-			bulk_g2s(s.w, w_image, W_BYTES, &s.w_bar);
-		}
-		__syncwarp();
-	}
 	mbar_wait(&s.w_bar, 0);
-	return *reinterpret_cast<volatile uint32_t*>(&s.tmem_base);
 }
-__device__ __forceinline__ void tile_teardown(TileSmem& s, uint32_t tmem_base) {
-	tc_fence_before();
-	__syncthreads();
-	if (threadIdx.x < 32) tmem_dealloc(tmem_base, TMEM_COLS);
+__device__ __forceinline__ TileCtx single_tile_ctx(TileSmem& s) {
+	TileCtx c;
+	c.a32 = s.a32; c.w_addr = smem_u32(s.w); c.row = threadIdx.x; c.bar_id = 0;
+	return c;
 }
 
 // ---- operand row stores ------------------------------------------------------------------------------
-// 8 consecutive fp16 (one 16-byte k-chunk) of this thread's row
+// 8 consecutive fp16 (one 16-byte k-chunk) of sample `row`
 __device__ __forceinline__ void store_chunk(uint8_t* base, uint32_t chunk, uint32_t row, uint4 v) {
-	*reinterpret_cast<uint4*>(base + chunk * (ROWS * 16) + row * 16) = v;
+	*reinterpret_cast<uint4*>(base + chunk * (ROWS * 16) + phys_row(row) * 16) = v;
 }
-__device__ __forceinline__ uint32_t pack_h2(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
-// ReLU after the fp16 conversion: rounding is monotone and 0 is exact, so max(cvt(x), 0) == cvt(max(x, 0)) — one packed
-// HMNMX2 per pair instead of two FMNMX.
-__device__ __forceinline__ uint32_t relu_pack(uint32_t a_bits, uint32_t b_bits) {
-	return pack_h2(__hmax2(__floats2half2_rn(__uint_as_float(a_bits), __uint_as_float(b_bits)), __floats2half2_rn(0.0f, 0.0f)));
+__device__ __forceinline__ uint4 load_chunk(const uint8_t* base, uint32_t chunk, uint32_t row) {
+	return *reinterpret_cast<const uint4*>(base + chunk * (ROWS * 16) + phys_row(row) * 16);
 }
-__device__ __forceinline__ uint32_t pack(uint32_t a_bits, uint32_t b_bits) {
-	return pack_h2(__floats2half2_rn(__uint_as_float(a_bits), __uint_as_float(b_bits)));
-}
-// two TMEM columns -> packed half2: fp32 accumulators are rounded here, fp16 accumulators (low half of each column) are just gathered
-template <bool ACC16> __device__ __forceinline__ uint32_t pack_acc(uint32_t a_bits, uint32_t b_bits) {
-	return ACC16 ? __byte_perm(a_bits, b_bits, 0x5410) : pack(a_bits, b_bits);
-}
-template <bool ACC16> __device__ __forceinline__ uint32_t relu_pack_acc(uint32_t a_bits, uint32_t b_bits) {
-	uint32_t p = pack_acc<ACC16>(a_bits, b_bits);
-	return pack_h2(__hmax2(*reinterpret_cast<__half2*>(&p), __floats2half2_rn(0.0f, 0.0f)));
+// A 16-wide output (this lane's 4 pairs of half `h`) -> k-chunks `chunk`, `chunk`+1 of the warp's own physical rows
+template <bool ACC16>
+__device__ __forceinline__ void store_out16(uint8_t* base, uint32_t chunk, uint32_t row, uint32_t h, const uint32_t* d) {
+	const uint32_t lane = row & 31u;
+	uint8_t* p = base + chunk * (ROWS * 16) + (64u * h + 16u * (row >> 5) + (lane >> 2)) * 16 + (lane & 3u) * 4;
+	*reinterpret_cast<uint32_t*>(p) = acc_pair<ACC16>(d, 0);
+	*reinterpret_cast<uint32_t*>(p + 8 * 16) = acc_pair<ACC16>(d, 1);
+	*reinterpret_cast<uint32_t*>(p + ROWS * 16) = acc_pair<ACC16>(d, 2);
+	*reinterpret_cast<uint32_t*>(p + ROWS * 16 + 8 * 16) = acc_pair<ACC16>(d, 3);
 }
 
-// Epilogue of a 64-wide hidden layer: TMEM fp32 [row][0..63] -> ReLU -> fp16 -> a64 row (8 chunks)
-template <bool ACC16 = false>
-__device__ __forceinline__ void epilogue_hidden(uint8_t* a64, uint32_t tmem_row, uint32_t row) {
-#pragma unroll
-	for (uint32_t q = 0; q < 2; ++q) {
-		uint32_t r[32];
-		tmem_ld16(tmem_row + q * 32, r);
-		tmem_ld16(tmem_row + q * 32 + 16, r + 16);
-		tmem_wait_ld();
-#pragma unroll
-		for (uint32_t j = 0; j < 4; ++j) {
-			uint4 c = make_uint4(relu_pack_acc<ACC16>(r[8 * j + 0], r[8 * j + 1]), relu_pack_acc<ACC16>(r[8 * j + 2], r[8 * j + 3]), relu_pack_acc<ACC16>(r[8 * j + 4], r[8 * j + 5]),
-			                     relu_pack_acc<ACC16>(r[8 * j + 6], r[8 * j + 7]));
-			store_chunk(a64, 4 * q + j, row, c);
-		}
-	}
-}
-
-// Runs the network on the tile's 128 rows whose grid features are already in c.a32 (chunks 0-3).
+// Runs the network on the tile's 128 samples whose grid features are already in the first layer's operand.
 //   density_only: stop after L2 (NerfNetwork::density)
-//   dens[8]: the 16 fp16 outputs of the density MLP (packed half2), rgb[8]: the 16 outputs of the rgb MLP.
-// `dw` = this row's warped view direction; its 16 SH values are evaluated between L2 and L3.
-// `phase` is the running parity of the tile's mma_bar (one flip per layer).
+//   dens[8]: the 16 fp16 outputs of the density MLP (packed half2), rgb[8]: the 16 outputs of the rgb MLP, both for sample c.row.
+// `dw` = this sample's warped view direction; its 16 SH values are evaluated between L2 and L3.
 // `a_first`: shared-window address of the first layer's operand when it does not live in c.a32 (the warp-specialised renderer's producers
-// write the grid features into their own double-buffered operand); 0 = c.a32.
+// write the grid features into their own operand); 0 = c.a32. `release`: an mbarrier to arrive on (one arrival) once every warp's first
+// layer has read that operand.
+// Operand space: chunks 0-3 the 32-wide layer inputs, 4-5 the rgb hand-back, 6-7 the density hand-back. On return the whole tile has
+// finished with the operand space, so the caller may overwrite any of it.
 template <bool ACC16 = false>
-__device__ __forceinline__ void run_network(const TileCtx& c, uint32_t& phase, V3 dw, bool density_only, uint32_t* dens, uint32_t* rgb, uint32_t a_first = 0) {
+__device__ __forceinline__ void run_network(const TileCtx& c, V3 dw, bool density_only, uint32_t* dens, uint32_t* rgb, uint32_t a_first = 0,
+                                            uint64_t* release = nullptr) {
 	const uint32_t row = c.row;
-	const uint32_t tmem_row = c.tmem + ((row & ~31u) << 16);  // lane field = first lane of this warp's quarter
-	const uint32_t a32 = smem_u32(c.a32), a64 = smem_u32(c.a64), w = c.w_addr;
+	const uint32_t a32 = smem_u32(c.a32), w = c.w_addr;
 	if (a_first == 0) a_first = a32;
-#define NSB_SYNC_ISSUE(N_, K_, A_, W_)                                  \
-	fence_async_smem();                                                 \
-	tc_fence_before();                                                  \
-	tile_sync(c);                                                       \
-	issue_converged<N_, K_, ACC16>(row, c.tmem, A_, w + W_, c.mma_bar); \
-	mbar_wait(c.mma_bar, phase); phase ^= 1;                            \
-	tc_fence_after();
-
-	NSB_SYNC_ISSUE(64, 32, a_first, W1_OFF)   // L1: grid features (32) -> 64
-	epilogue_hidden<ACC16>(c.a64, tmem_row, row);
-	NSB_SYNC_ISSUE(16, 64, a64, W2_OFF)   // L2: a64 (64) -> 16
-	{
-		uint32_t r[16];
-		tmem_ld16(tmem_row, r);
-		tmem_wait_ld();
-#pragma unroll
-		for (int i = 0; i < 8; ++i) dens[i] = pack_acc<ACC16>(r[2 * i], r[2 * i + 1]);
+	fence_async_smem();
+	tile_sync(c);  // every sample's grid features are in place
+#pragma unroll 1
+	for (uint32_t h = 0; h < 2; ++h) {
+		Acc<64, ACC16> x;
+		Acc<16, ACC16> o;
+		layer_ss<64, 32, ACC16>(x.r, a_first + h * 64 * 16, w + W1_OFF);  // L1: grid features (32) -> 64
+		layer_rs<16, 64, ACC16>(o.r, x.r, w + W2_OFF);                    // L2: 64 -> 16
+		store_out16<ACC16>(c.a32, 6, row, h, o.r);
 	}
-	if (density_only) { tc_fence_before(); return; }
-	// rgb-network input: rows 0-15 = density MLP output, 16-31 = SH (nerf_network_full.h:52,67,79)
+	__syncwarp();
+	{
+		const uint4 d0 = load_chunk(c.a32, 6, row), d1 = load_chunk(c.a32, 7, row);
+		dens[0] = d0.x; dens[1] = d0.y; dens[2] = d0.z; dens[3] = d0.w; dens[4] = d1.x; dens[5] = d1.y; dens[6] = d1.z; dens[7] = d1.w;
+	}
+	tile_sync(c);  // every warp's first layer has read its operand
+	if (density_only) return;
+	if (release && row == 0) mbar_arrive(release);
+	// rgb-network input: columns 0-15 = density MLP output, 16-31 = SH (nerf_network_full.h:52,67,79)
 	__half2 sh[8];
-	encode_sh4(dw, sh);  // tcnn SphericalHarmonics of the (mapped) direction: rows 16-31 of the rgb network input
+	encode_sh4(dw, sh);  // tcnn SphericalHarmonics of the (mapped) direction
 	store_chunk(c.a32, 0, row, make_uint4(dens[0], dens[1], dens[2], dens[3]));
 	store_chunk(c.a32, 1, row, make_uint4(dens[4], dens[5], dens[6], dens[7]));
 	store_chunk(c.a32, 2, row, make_uint4(pack_h2(sh[0]), pack_h2(sh[1]), pack_h2(sh[2]), pack_h2(sh[3])));
 	store_chunk(c.a32, 3, row, make_uint4(pack_h2(sh[4]), pack_h2(sh[5]), pack_h2(sh[6]), pack_h2(sh[7])));
-	NSB_SYNC_ISSUE(64, 32, a32, W3_OFF)   // L3: a32 -> 64
-	epilogue_hidden<ACC16>(c.a64, tmem_row, row);
-	NSB_SYNC_ISSUE(64, 64, a64, W4_OFF)   // L4: a64 -> 64
-	epilogue_hidden<ACC16>(c.a64, tmem_row, row);
-	NSB_SYNC_ISSUE(16, 64, a64, W5_OFF)   // L5: a64 -> 16
-	{
-		uint32_t r[16];
-		tmem_ld16(tmem_row, r);
-		tmem_wait_ld();
-#pragma unroll
-		for (int i = 0; i < 8; ++i) rgb[i] = pack_acc<ACC16>(r[2 * i], r[2 * i + 1]);
+	fence_async_smem();
+	tile_sync(c);
+#pragma unroll 1
+	for (uint32_t h = 0; h < 2; ++h) {
+		Acc<64, ACC16> x, y;
+		Acc<16, ACC16> o;
+		layer_ss<64, 32, ACC16>(x.r, a32 + h * 64 * 16, w + W3_OFF);  // L3: 32 -> 64
+		layer_rs<64, 64, ACC16>(y.r, x.r, w + W4_OFF);                // L4: 64 -> 64
+		layer_rs<16, 64, ACC16>(o.r, y.r, w + W5_OFF);                // L5: 64 -> 16
+		store_out16<ACC16>(c.a32, 4, row, h, o.r);
 	}
-	tc_fence_before();
-#undef NSB_SYNC_ISSUE
-}
-__device__ __forceinline__ TileCtx single_tile_ctx(TileSmem& s, uint32_t tmem_base) {
-	TileCtx c;
-	c.a32 = s.a32; c.a64 = s.a64; c.w_addr = smem_u32(s.w); c.mma_bar = &s.mma_bar; c.tmem = tmem_base; c.row = threadIdx.x; c.bar_id = 0;
-	return c;
+	__syncwarp();
+	{
+		const uint4 r0 = load_chunk(c.a32, 4, row), r1 = load_chunk(c.a32, 5, row);
+		rgb[0] = r0.x; rgb[1] = r0.y; rgb[2] = r0.z; rgb[3] = r0.w; rgb[4] = r1.x; rgb[5] = r1.y; rgb[6] = r1.z; rgb[7] = r1.w;
+	}
+	tile_sync(c);
 }
 
 }  // namespace tc

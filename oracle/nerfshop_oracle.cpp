@@ -439,8 +439,8 @@ void encode_sh4(V3 dw, uint16_t* out /*16*/) {
 // Accumulator policy of the fully fused MLPs (orc_set_mlp_policy):
 //   1 (default) half accumulator fragments: tiny-cuda-nn's FullyFusedMLP of that era runs wmma m16n16k16 with __half accumulators (SURVEY.md
 //     Appendix B; the submodule is absent, so unverifiable here): the running sum is rounded to fp16 after every k-chunk of 16 (products and
-//     the 16-term partial sum inside one MMA are kept wide). The CUDA path's default (tcgen05 kind::f16 with D = F16) reproduces it 99.9 % bit for bit;
-//   0 wide: every output is the exactly-rounded dot product (double accumulate, one rounding to fp16) — what fp32 TMEM accumulators
+//     the 16-term partial sum inside one MMA are kept wide). The CUDA path's default (wgmma with an fp16 D) reproduces it 99.9 % bit for bit;
+//   0 wide: every output is the exactly-rounded dot product (double accumulate, one rounding to fp16) — what fp32 accumulators
 //     (NSB_MLP_ACC_F32) approximate to 2-4 fp16 ulps.
 // tests/test_mlp_policy.py measures how far the two are apart in the framebuffer (up to 1e-2 on 0.02 % of the pixels).
 int g_mlp_policy = 1;

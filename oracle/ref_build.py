@@ -274,7 +274,7 @@ def build(force: bool = False, verbose: bool = False):
 
 
 def build_cuda(force: bool = False):
-    """The same reference sources compiled by nvcc for sm_100a (oracle/ref_driver_cuda.cu): the reference's kernels and host loop
+    """The same reference sources compiled by nvcc for sm_90a (oracle/ref_driver_cuda.cu): the reference's kernels and host loop
     run on the GPU. Returns the library path, or None when /root/reference is absent and no prebuilt library exists."""
     if not available():
         return LIB_CUDA if os.path.exists(LIB_CUDA) else None
@@ -284,7 +284,7 @@ def build_cuda(force: bool = False):
     gen = os.path.join(OUT_DIR, "gen_cuda")
     shutil.rmtree(gen, ignore_errors=True)
     extract_all(gen)
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "--extended-lambda", "--expt-relaxed-constexpr",
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "--extended-lambda", "--expt-relaxed-constexpr",
            "-Xcompiler", "-fPIC", "-shared", "-w"] + (["-ccbin", "/usr/bin/g++"] if os.path.exists("/usr/bin/g++") else []) + [
            "-I", SHIM, "-I", gen, "-I", os.path.join(REF, "include"), "-I", os.path.join(REF, "src"), DRIVER_CUDA, "-o", LIB_CUDA]
     res = subprocess.run(cmd, capture_output=True, text=True)

@@ -1,4 +1,4 @@
-// ref_driver_cuda.cu — the reference's OWN CUDA render path, compiled by nvcc for sm_100a (oracle/_ref/libnerfshop_ref_cuda.so).
+// ref_driver_cuda.cu — the reference's OWN CUDA render path, compiled by nvcc for sm_90a (oracle/_ref/libnerfshop_ref_cuda.so).
 //
 // TEST / BASELINE INFRASTRUCTURE ONLY. Same reference sources as oracle/ref_driver.cpp (see ref_build.py EXTRACTS and
 // ref_common.inl) — Testbed::render_nerf, NerfTracer::{init_rays_from_camera, trace, enlarge}, every kernel they launch, the

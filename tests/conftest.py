@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `pytest -m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: `pytest -m gpu`)")
 
 
 @pytest.fixture(scope="session")
@@ -33,7 +33,7 @@ def oracle(scene):
 
 @pytest.fixture(scope="session")
 def built_lib():
-    """The sm_100a library, built in-tree if needed (nvcc cross-compiles without a GPU)."""
+    """The sm_90a library, built in-tree if needed (nvcc cross-compiles without a GPU)."""
     from nerfshop_b200 import build
 
     return build.build()

@@ -1,4 +1,4 @@
-"""CPU tests of the drop-in boundary: the C-ABI library builds for sm_100a, loads, and exports exactly
+"""CPU tests of the drop-in boundary: the C-ABI library builds for sm_90a, loads, and exports exactly
 the symbols include/nerfshop_b200.h declares (no compute calls: there is no GPU in CI)."""
 import ctypes as C
 import os

@@ -7,9 +7,9 @@ import pytest
 
 from nerfshop_b200 import abi
 from nerfshop_b200 import synthetic as syn
-from oracle import ref
+from ref_golden import ref
 
-pytestmark = pytest.mark.skipif(not ref.available(), reason="oracle/_ref not built and /root/reference absent")
+pytestmark = pytest.mark.skipif(not ref.usable("test_frame_extras_cpu"), reason="neither oracle/_ref nor stored reference results (tests/golden/ref/)")
 
 W, H = 112, 63
 CASES = {
@@ -97,6 +97,9 @@ def test_ray_stream_with_lens_distortion(scene, oracle):
     MS = 48
     rec_o, idx_o, cnt_o = oracle.march_trace(f, pix, MS)
     rec_r, ray_r, cnt_r, alive_r = ref.march_trace(f, occ, pix, MS)
+    frac = ref.fraction(cnt_r)  # a stored reference result keeps a seeded sample of the rays: compare on those
+    rec_o, rec_r = ref.match(rec_o, rec_r)
+    cnt_o, cnt_r = ref.match(cnt_o, cnt_r)
     cnt_o = np.minimum(cnt_o, MS)
     assert (cnt_o > 0).mean() > 0.3
     # Newton undistortion + sincosf: rays agree to float rounding, so a handful of rays may gain or lose a sample at a cell face
@@ -135,10 +138,13 @@ def test_random_general_cameras_ray_stream(scene, oracle, seed):
     MS = 8
     rec_o, idx_o, cnt_o = oracle.march_trace(f, pix, MS)
     rec_r, ray_r, cnt_r, alive_r = ref.march_trace(f, occ, pix, MS)
+    frac = ref.fraction(cnt_r)  # a stored reference result keeps a seeded sample of the rays: compare on those
+    rec_o, rec_r = ref.match(rec_o, rec_r)
+    cnt_o, cnt_r = ref.match(cnt_o, cnt_r)
     cnt_o = np.minimum(cnt_o, MS)
     both = (cnt_o > 0) & (cnt_r > 0)
     d = np.abs((rec_o[both, 0, 0] + rec_o[both, 0, 1]).astype(np.float32) - rec_r[both, 0, 7])
     print(f"\nseed {seed}: {both.sum()} rays with samples; counts equal on {(cnt_o == cnt_r).mean() * 100:.2f} %; first-sample t identical on {(d == 0).mean() * 100:.2f} %, max diff {d.max():.2e}")
-    assert both.sum() > 300
+    assert both.sum() > 300 * frac
     assert (cnt_o == cnt_r).mean() > 0.98
     assert (d == 0).mean() > 0.95 and (d > 1e-4).mean() < 0.02

@@ -3,7 +3,7 @@ membrane residual -> max-splat, then EMA merge and bitfield rebuild) against the
 Testbed::update_density_grid_nerf_operator (testbed_nerf.cu:3533-3639).
 
 Tolerances: cell selection, sample positions, operator mapping and the splat/EMA/bitfield logic are integer/pinned-fp32 work and
-must agree exactly; the density value goes through the fp16 MLP (tcgen05 fp32 accumulation vs the oracle's wide accumulation:
+must agree exactly; the density value goes through the fp16 MLP (wgmma fp32 accumulation vs the oracle's wide accumulation:
 raw outputs within a few fp16 ulps, test_gpu_parity) and __expf, so a cell's value may differ by the fp16 spacing of the raw
 output: |ln(gpu/cpu)| <= 4 ulp_fp16(raw) <= 4 * 2^-7 for |raw| < 8. Bitfield bytes may differ only where a cell of that byte sits
 within that tolerance of the threshold."""

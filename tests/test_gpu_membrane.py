@@ -1,4 +1,4 @@
-"""§8(f)-4 on the GPU: nsb_poisson_boundary (directions on the host, inference on tcgen05, activation + SH9 fit on the device) and
+"""§8(f)-4 on the GPU: nsb_poisson_boundary (directions on the host, inference on wgmma, activation + SH9 fit on the device) and
 nsb_cage_set_membrane (the gamma-coordinate blend into the operator's device arrays) against the oracle.
 Tolerances: colours/densities pass the fp16 MLP (raw outputs within a few fp16 ulps) and expf -> density within 4 ulp_fp16(raw)
 relative, SH coefficients (means of ~100 colours in (0,1) times |Y| <= 1.1, scaled by 4pi) within 2e-3. The blend is pinned fp32 on

@@ -33,7 +33,7 @@ def _ulp_close(got_u16, ref_u16, ulps=2, atol=1e-3):
 
 
 def test_library_loaded_is_the_cuda_extension(renderer):
-    # the product path has no fallback: the context exists only if libnerfshop_b200.so loaded and found an sm_100 device
+    # the product path has no fallback: the context exists only if libnerfshop_b200.so loaded and found an sm_90 device
     assert renderer.ctx
     with open("/proc/self/maps") as fh:
         assert "libnerfshop_b200.so" in fh.read()

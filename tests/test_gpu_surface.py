@@ -11,7 +11,7 @@ from edit_fixtures import e3
 from nerfshop_b200 import abi, editing
 from nerfshop_b200 import synthetic as syn
 from oracle import oracle as orc
-from oracle import ref, ref_build
+from ref_golden import ref
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -72,7 +72,7 @@ def test_cpp_shim_renders_the_same_frame(scene, renderer, built_lib, tmp_path):
     assert np.array_equal(got[4 * n:].reshape(90, 160), depth.cpu().numpy())
 
 
-@pytest.mark.skipif(ref_build.build_cuda() is None, reason="oracle/_ref CUDA library absent")
+@pytest.mark.skipif(not ref.cuda_usable("test_gpu_surface"), reason="neither oracle/_ref nor stored reference results (tests/golden/ref/)")
 @pytest.mark.parametrize("mode,level", [(abi.NSB_RENDER_SHADE, 0), (abi.NSB_RENDER_POSITIONS, 1), (abi.NSB_RENDER_POSITIONS, 0)])
 def test_show_accel_override_identical_to_reference(scene, renderer, mode, level):
     """m_nerf.show_accel >= 0: alpha = 1 for every sample (testbed_nerf.cu:788-790), Positions mode colours the occupancy cells (:913-923)."""

@@ -1,6 +1,6 @@
 """Pins oracle/ (and the product's host geometry) to oracle/_ref = the reference's OWN sources compiled for the CPU.
 
-oracle/_ref/libnerfshop_ref.so is built by oracle/ref_build.py from /root/reference (unmodified headers, src/common_nerf.cu, and the
+oracle/_ref/libnerfshop_ref.so is built by oracle/ref_build.py from the reference's sources (unmodified headers, src/common_nerf.cu, and the
 functions listed in ref_build.EXTRACTS — Testbed::render_nerf, NerfTracer::trace, init_rays_from_camera, every kernel they launch,
 interpolate_tet, translate_in_box, compute_residual_poisson_kernel, Cage::compute_mvc over mvc.h, TetMesh::update_local_rotations
 over svd3.h, TetMesh::build_tet_grid) behind stand-ins for the absent submodules (oracle/ref_shim/). Only tiny-cuda-nn's network is
@@ -19,9 +19,9 @@ from edit_fixtures import e1, e3, make_cage
 from nerfshop_b200 import abi, editing
 from nerfshop_b200 import synthetic as syn
 from oracle import oracle as orc
-from oracle import ref
+from ref_golden import ref
 
-pytestmark = pytest.mark.skipif(not ref.available(), reason="oracle/_ref not built and /root/reference absent")
+pytestmark = pytest.mark.skipif(not ref.usable("test_oracle_vs_ref"), reason="neither oracle/_ref nor stored reference results (tests/golden/ref/)")
 
 
 _a = 0.4
@@ -74,14 +74,18 @@ def test_srgb_sh9_activations():
     # the oracle's composite uses the same formulas; here the numpy restatement of each is the reference function itself
     s = rng.uniform(0, 1.2, 50000).astype(np.float32)
     lin = ref.srgb_to_linear(s)
+    s, lin = ref.match(s, lin)  # a stored reference result keeps a seeded sample of the inputs' rows: compare on those
     want = np.where(s <= 0.04045, s / np.float32(12.92), np.power((s + np.float32(0.055)) / np.float32(1.055), np.float32(2.4)))
     assert np.abs(lin - want).max() < 2e-6
     rgb, dens = ref.activations(x, abi.NSB_ACT_LOGISTIC)
-    assert np.abs(rgb - 1.0 / (1.0 + np.exp(-x.astype(np.float64)))).max() < 1e-6
+    xs, rgb = ref.match(x, rgb)
+    assert np.abs(rgb - 1.0 / (1.0 + np.exp(-xs.astype(np.float64)))).max() < 1e-6
     _, dens = ref.activations(x, abi.NSB_ACT_EXPONENTIAL)
-    assert np.allclose(dens, np.exp(x.astype(np.float64)), rtol=2e-6)
+    xs, dens = ref.match(x, dens)
+    assert np.allclose(dens, np.exp(xs.astype(np.float64)), rtol=2e-6)
     rgb, _ = ref.activations(x, abi.NSB_ACT_EXPONENTIAL)
-    assert np.allclose(rgb, np.exp(np.clip(x.astype(np.float64), -10, 10)), rtol=2e-6)
+    xs, rgb = ref.match(x, rgb)
+    assert np.allclose(rgb, np.exp(np.clip(xs.astype(np.float64), -10, 10)), rtol=2e-6)
 
 
 # ---- ray generation + occupancy stepping: init_rays_with_payload_kernel_nerf, advance_pos_nerf, generate_next_nerf_network_inputs --
@@ -93,12 +97,15 @@ def test_march_vs_reference_kernels(scene, oracle, cam_index, spp):
     pix = np.random.default_rng(cam_index).choice(W * H, 4000, replace=False).astype(np.uint32)
     rec_o, idx_o, cnt_o = oracle.march_trace(f, pix, MS)
     rec_r, ray_r, cnt_r, alive = ref.march_trace(f, occ, pix, MS)
+    frac = ref.fraction(cnt_r)  # a stored reference result keeps a seeded sample of the rays: compare on those
+    rec_o, rec_r = ref.match(rec_o, rec_r)
+    cnt_o, cnt_r = ref.match(cnt_o, cnt_r)
     # same rays enter, same number of occupied samples on every ray
     assert np.array_equal(np.minimum(cnt_o, MS), cnt_r)
     amin, amax = np.array(list(f.train_aabb_min), np.float32), np.array(list(f.train_aabb_max), np.float32)
     total = bad_t = bad_p = bad_dt = 0
     max_ulp = 0
-    for k in range(pix.size):
+    for k in range(cnt_r.size):
         c = int(cnt_r[k])
         if c == 0:
             continue
@@ -109,7 +116,7 @@ def test_march_vs_reference_kernels(scene, oracle, cam_index, spp):
         bad_p += int((d > 0).any(axis=1).sum())
         max_ulp = max(max_ulp, float(d.max()) / 2.0 ** -24)
     print(f"\ncam {cam_index} spp {spp}: {total} samples; t-stream mismatches {bad_t}; warped positions differing {bad_p} ({100.0 * bad_p / total:.1f} %, max {max_ulp:.1f} ulp of 1.0)")
-    assert total > 50_000
+    assert total > 50_000 * frac
     # the dt lattice (t, dt, and with them the occupancy cell sequence) is bit-identical to the reference's kernels
     assert bad_t == 0
     # positions: identical up to the FMA contraction of the camera matrix product / normalisation (compiler's choice), i.e. a few ulps
@@ -185,10 +192,14 @@ def test_map_rays_and_poisson_vs_reference_kernels(scene):
     d = rng.standard_normal((n, 3)).astype(np.float32)
     c[:, 4:] = (d / np.linalg.norm(d, axis=1, keepdims=True) + 1) * 0.5
     co, mo = o.map_rays(c)
-    cr, mr = ref.map_rays(ops, c)
-    moved = (co[:, :3] != c[:, :3]).any(axis=1)
-    assert moved.sum() > 5000 and mo.sum() > 300
-    flips = int((mo != mr).sum()) + int(((cr[:, :3] != c[:, :3]).any(axis=1) != moved).sum())
+    cr0, mr = ref.map_rays(ops, c)
+    frac = ref.fraction(cr0)  # a stored reference result keeps a seeded sample of the coordinates: compare on those
+    co, cr = ref.match(co, cr0)
+    mo, mr = ref.match(mo, mr)
+    cs, _ = ref.match(c, cr0)
+    moved = (co[:, :3] != cs[:, :3]).any(axis=1)
+    assert moved.sum() > 5000 * frac and mo.sum() > 300 * frac
+    flips = int((mo != mr).sum()) + int(((cr[:, :3] != cs[:, :3]).any(axis=1) != moved).sum())
     dpos, ddir = np.abs(co[:, :3] - cr[:, :3]) / 2.0 ** -24, np.abs(co[:, 4:] - cr[:, 4:]) / 2.0 ** -24  # warped values live in [0, 1]: in ulps of 1.0
     big = (dpos > 64).any(axis=1)  # a sample that landed in a different tet on a shared face would show as a large jump
     print(f"\nmap_rays: {moved.sum()} moved, {mo.sum()} masked; mask/moved flips {flips}; position max {dpos.max():.1f} ulp ({(dpos > 0).any(axis=1).sum()} differ), direction max {ddir.max():.1f} ulp; {big.sum()} large jumps")
@@ -196,8 +207,12 @@ def test_map_rays_and_poisson_vs_reference_kernels(scene):
     assert np.percentile(dpos.max(axis=1), 99.9) <= 8 and np.percentile(ddir.max(axis=1), 99.9) <= 8
     sh_o, od_o, rd_o = o.poisson_residuals(c)
     sh_r, od_r, rd_r = ref.poisson_residuals(ops, c)
+    frac = ref.fraction(od_r)
+    sh_o, sh_r = ref.match(sh_o, sh_r)
+    od_o, od_r = ref.match(od_o, od_r)
+    rd_o, rd_r = ref.match(rd_o, rd_r)
     inside = od_o != 0
-    assert inside.sum() > 2000 and np.array_equal(inside, od_r != 0) or abs(int(inside.sum()) - int((od_r != 0).sum())) <= 2
+    assert inside.sum() > 2000 * frac and np.array_equal(inside, od_r != 0) or abs(int(inside.sum()) - int((od_r != 0).sum())) <= 2
     both = inside & (od_r != 0)
     assert np.allclose(od_o[both], od_r[both], rtol=2e-5, atol=1e-5) and np.allclose(rd_o[both], rd_r[both], rtol=2e-5, atol=1e-5)
     assert np.allclose(sh_o[both], sh_r[both], rtol=2e-5, atol=2e-5)
@@ -385,19 +400,22 @@ def test_occupancy_update_vs_reference_update_density_grid_nerf_operator(scene, 
         grid_o, bits_o, mean_o = o.update_density_grid(u, grid_o)
         grid_r, bits_r, mean_r = ref.update_density_grid(u, grid_r, density, ops=ops)
         rng.advance(); rng.advance()  # m_rng.advance() after each of the two sample-generation launches
-        touched = (grid_o > 0) | (grid_r > 0)
-        same = grid_o == grid_r
-        rel = np.abs(grid_o - grid_r)[touched] / np.maximum(grid_r[touched], 1e-12)
+        frac = ref.fraction(grid_r)  # a stored reference result keeps a seeded sample of the cells: compare on those
+        go, gr = ref.match(grid_o, grid_r)
+        bo, br = ref.match(bits_o, bits_r)
+        touched = (go > 0) | (gr > 0)
+        same = go == gr
+        rel = np.abs(go - gr)[touched] / np.maximum(gr[touched], 1e-12)
         print(f"\n{'E3+affine' if edited else 'no operators'} step {step}: {touched.sum()} cells touched, {(~same).sum()} differ (max rel {rel.max() if rel.size else 0:.2e}); "
-              f"mean {mean_o:.6g} vs {mean_r:.6g}; bitfield bytes differing {np.count_nonzero(bits_o != bits_r)}")
-        assert touched.sum() > 50_000
-        assert np.array_equal(grid_o > 0, grid_r > 0), "same cells touched"
+              f"mean {mean_o:.6g} vs {mean_r:.6g}; bitfield bytes differing {np.count_nonzero(bo != br)}")
+        assert touched.sum() > 50_000 * frac
+        assert np.array_equal(go > 0, gr > 0), "same cells touched"
         # positions may differ by an ulp where the operators map them (gcc vs nvcc contraction of the tet barycentrics, DESIGN.md section 3): the raw
         # fp16 density of such a sample moves by a few fp16 ulps (1 ulp = 1e-3 relative) — a handful of cells in 10^5
         # and a sample within an ulp of a tet face may be mapped by one build and not by the other: at most a few cells in 10^5 differ freely
         assert (~same).sum() <= 1e-4 * touched.sum() + 2 and (rel > 1e-2).sum() <= 3
         assert abs(mean_o - mean_r) <= 1e-6 * max(mean_r, 1e-6) + 1e-9
-        assert np.count_nonzero(bits_o != bits_r) <= 2
+        assert np.count_nonzero(bo != br) <= 2
 
 
 def test_accumulate_and_tonemap_vs_reference_kernels():
@@ -414,8 +432,9 @@ def test_accumulate_and_tonemap_vs_reference_kernels():
             fr = (frame * np.float32(1.0 + 0.1 * spp)).astype(np.float32)
             acc_o = orc.accumulate(fr, acc_o, spp, cs)
             acc_r = ref.accumulate(fr, acc_r, spp, cs)
-            worst_acc = max(worst_acc, float(np.abs(acc_o - acc_r).max()))
-            assert np.allclose(acc_o, acc_r, rtol=2e-6, atol=2e-7), (cs, spp)
+            a_o, a_r = ref.match(acc_o, acc_r)  # a stored reference result keeps a seeded sample of the rows: compare on those
+            worst_acc = max(worst_acc, float(np.abs(a_o - a_r).max()))
+            assert np.allclose(a_o, a_r, rtol=2e-6, atol=2e-7), (cs, spp)
         for curve in (abi.NSB_TONEMAP_IDENTITY, abi.NSB_TONEMAP_ACES, abi.NSB_TONEMAP_HABLE, abi.NSB_TONEMAP_REINHARD):
             for out_cs, clamp, exposure in ((abi.NSB_COLOR_SRGB, 1, 0.0), (abi.NSB_COLOR_LINEAR, 0, 0.7), (abi.NSB_COLOR_SRGB, 0, -1.3)):
                 p = abi.NsbTonemap()
@@ -423,6 +442,7 @@ def test_accumulate_and_tonemap_vs_reference_kernels():
                 p.background_color[:] = (0.2, 0.4, 0.6, 0.8)
                 t_o = orc.tonemap(acc_o, p)
                 t_r = ref.tonemap(acc_r, exposure, list(p.background_color), cs, out_cs, curve, bool(clamp))
+                t_o, t_r = ref.match(t_o, t_r)
                 err = np.abs(t_o - t_r) / np.maximum(1.0, np.abs(t_r))
                 finite = np.isfinite(t_r)
                 assert np.array_equal(np.isfinite(t_o), finite)

@@ -1,4 +1,4 @@
-"""Writes profiles/r2_mlp_accumulator_policy.txt: the oracle's frames under the two MLP accumulator policies (wide vs wmma __half fragments)."""
+"""Writes profiles/mlp_accumulator_policy.txt (measurement output, not committed): the oracle's frames under the two MLP accumulator policies (wide vs wmma __half fragments)."""
 import os
 import sys
 
@@ -26,8 +26,9 @@ for name, cam in cams:
                  f"samples {sa.n_samples} vs {sb.n_samples}")
 lines += ["", "Reading: the two policies agree to ~4e-5 on average but NOT within the 1e-3 RGBA contract everywhere: 0.02 % of the pixels move by up to 1e-2",
           "(a 1-ulp change of the raw fp16 density is 0.1-0.8 % of sigma = exp(raw); it can move an early termination or the max-weight sample).",
-          "The CUDA path therefore follows the reference's policy by default (fp16 TMEM accumulators, 99.9 % bit-equal to this emulation) and exposes the other",
+          "The CUDA path therefore follows the reference's policy by default (fp16 wgmma accumulators) and exposes the other",
           "(nsb_set_mlp_accumulator); see DESIGN.md section 3."]
-out = os.path.join(ROOT, "profiles", "r2_mlp_accumulator_policy.txt")
+out = os.path.join(ROOT, "profiles", "mlp_accumulator_policy.txt")
+os.makedirs(os.path.dirname(out), exist_ok=True)
 open(out, "w").write("\n".join(lines) + "\n")
 print("\n".join(lines))
