@@ -31,6 +31,7 @@ struct RayRec { uint32_t pix; float t; };  // a ray that entered the AABB and fo
 enum { ST_RAYS = 0, ST_ALIVE = 1, ST_HIT = 2, ST_SAMPLES = 3, ST_OLD = 4, ST_ROUNDS = 5, ST_CYC_ACQUIRE = 6, ST_CYC_ENCODE = 7, ST_CYC_MLP = 8,
        ST_CYC_COMPOSITE = 9, ST_CYC_TOTAL = 10, ST_CTAS = 11, ST_N = 12 };
 constexpr int DDA_BUDGET = 8;   // empty voxels a lane may skip per MLP round before it yields (latency bound of a round)
+constexpr int REFILL_THR = 2;   // the free lanes of a warp refill once at most this many of its rays are alive
 
 // tile slot -> pixel: the four warps of a 16x8 tile each cover an 8x4 block so that the 32 lanes of a warp stay
 // spatially compact (coherent hash-grid and occupancy lookups)
@@ -147,36 +148,20 @@ __device__ __forceinline__ void encode_to_a32(uint8_t* a32, const DevModel& m, b
 __device__ __forceinline__ float h_lo(uint32_t packed) { return __half2float(__ushort_as_half((unsigned short)(packed & 0xffffu))); }
 __device__ __forceinline__ float h_hi(uint32_t packed) { return __half2float(__ushort_as_half((unsigned short)(packed >> 16))); }
 
-// position of the k-th (0-based) set bit of m; popc(m) > k
-__device__ __forceinline__ uint32_t nth_set_bit(uint32_t m, uint32_t k) {
-	uint32_t p = 0;
-#pragma unroll
-	for (uint32_t s = 16; s >= 1; s >>= 1) {
-		const uint32_t c = (uint32_t)__popc((m >> p) & ((1u << s) - 1u));
-		if (k >= c) { k -= c; p += s; }
-	}
-	return p;
-}
-
-// Stage 2 (persistent; a tile = 128 threads = 128 ray slots = 128 MMA rows, NSB_TILES tiles per CTA): every round each live ray contributes
+// Stage 2 (persistent; a tile = 128 threads = 128 ray slots = 128 MMA rows, RENDER_TILES tiles per CTA): every round each live ray contributes
 // ONE sample; samples go deform -> hash encode -> wgmma MLPs -> composite inside the SM; a finished ray is shaded
 // into the framebuffer and its slot refilled from the queue (warp-convergent fetch of consecutive entries, so rays that
 // were refilled together — neighbouring pixels that die on the same surface — stay together in a warp).
 // Per-slot ray state parked in shared memory (SoA: lane-contiguous, conflict-free). Only the acquire and composite phases
 // touch it, so it does not occupy registers while the thread gathers hash-grid features and walks the MLP layers.
 enum { R_OX = 0, R_OY, R_OZ, R_DX, R_DY, R_DZ, R_T, R_CR, R_CG, R_CB, R_CA, R_DEPTH, R_MAXW, R_FIELDS };
-// One CTA per SM holds NSB_TILES independent tiles (a tile = 128 threads = 128 ray slots = one warpgroup). The tiles share the 20 KB
+// One CTA per SM holds RENDER_TILES independent tiles (a tile = 128 threads = 128 ray slots = one warpgroup). The tiles share the 20 KB
 // weight image — four separate CTAs would hold four copies — which matters because shared memory is carved out of the same
 // 256 KB as the L1 that serves the hash-grid gathers.
 // How many: the register file's worth. Frames without operators: 6 tiles (24 warps per SM, 80 registers per thread, 155 KB of shared memory);
-// the default fp16-accumulator build does not spill, the fp32 one spills 72 B per thread. Frames with operators carry the deform / membrane
-// state: 5 tiles (96 registers; 124-148 B spilled per thread with the wgmma layer chain). Other tile counts are not measured on the H100.
-#ifndef NSB_TILES
-#define NSB_TILES 6
-#endif
-#ifndef NSB_TILES_OPS
-#define NSB_TILES_OPS 5
-#endif
+// the default fp16-accumulator build does not spill, the fp32 one spills 50 B per thread. Frames with operators carry the deform / membrane
+// state: 5 tiles (96 registers; 110-134 B spilled per thread with the wgmma layer chain). Other tile counts are not measured on the H100.
+constexpr int RENDER_TILES = 6, RENDER_TILES_OPS = 5;
 struct TileBlock {
 	union {
 		uint8_t a64[tc::A64_BYTES];
@@ -191,31 +176,18 @@ struct __align__(128) RenderSmemT {
 	uint64_t w_bar;
 	uint32_t pad[2];
 };
-__host__ __device__ constexpr int render_tiles(bool ops) { return ops ? NSB_TILES_OPS : NSB_TILES; }
-static_assert(NSB_TILES >= 1 && NSB_TILES <= 8 && NSB_TILES_OPS >= 1 && NSB_TILES_OPS <= 8, "1..8 tiles (warpgroups) per CTA");
+__host__ __device__ constexpr int render_tiles(bool ops) { return ops ? RENDER_TILES_OPS : RENDER_TILES; }
+static_assert(RENDER_TILES >= 1 && RENDER_TILES <= 8 && RENDER_TILES_OPS >= 1 && RENDER_TILES_OPS <= 8, "1..8 tiles (warpgroups) per CTA");
 
 // OPS = false: the instantiation for frames without edit operators (f.apply_ops == 0 or no operator uploaded) carries none of the deform /
 // membrane code in its hot loop (the loop has to fit the instruction cache).
 // ACC16: the MLP accumulator policy (nsb_set_mlp_accumulator): fp16 wgmma accumulators, like the reference's wmma __half fragments.
-// experiment switches (tools/ab_kernels.py variants): compile a feature of the fused kernel out to measure what its presence costs the default path
-#ifndef NSB_X_ACCEL
-#define NSB_X_ACCEL 1
-#endif
-#ifndef NSB_X_GLOW
-#define NSB_X_GLOW 1
-#endif
-#ifndef NSB_X_RAYOD
-#define NSB_X_RAYOD 1
-#endif
-#ifndef NSB_X_HELP
-#define NSB_X_HELP 0  // helper lanes: an experiment, compiled out of the product (their presence alone changes register allocation / code layout); `build.build_variant("helpers", ["NSB_X_HELP=1"])` is the experiment build NSB_HELPERS acts on
-#endif
 template <bool OPS, bool ACC16>
 __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(const DevFrame f, const DevModel m, const uint8_t* __restrict__ bitfield,
                                                       const DevOp* __restrict__ ops, const int n_ops, const int any_poisson,
                                                       float4* __restrict__ fb, float* __restrict__ depth_out, const RayRec* __restrict__ list,
                                                       const float* __restrict__ ray_od, const uint32_t* __restrict__ n_queued_ptr, uint32_t* fetch_counter,
-                                                      unsigned long long* __restrict__ stats, const int refill_thr, const int dda_flags) {
+                                                      unsigned long long* __restrict__ stats) {
 	extern __shared__ __align__(128) uint8_t smem_raw[];
 	constexpr int TILES = render_tiles(OPS);
 	using RenderSmem = RenderSmemT<TILES>;
@@ -235,29 +207,10 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 	C.a32 = TB.a32; C.w_addr = tc::smem_u32(RS.w); C.row = tid;
 	C.bar_id = 1 + tile;
 
-	const int dda_budget = dda_flags & 0xffff;
-	// Helper lanes (frames without operators). A round costs the same ~20 K cycles whether 32 or 3 lanes of a warp carry a sample, and a warp only
-	// refills once it is down to refill_thr rays, so the lanes WITHOUT a ray are lent to the rays that found a sample this round: each such ray gets up
-	// to HELP_DEPTH of them, and helper j evaluates the ray's j-th NEXT sample (t advanced j times by calc_dt, its own occupancy test) through the
-	// encode and the MLPs. The owner lane then composites its own sample and, in march order, the helpers' — up to the first one that was not an
-	// occupied in-bounds sample, where the ordinary march resumes next round. Samples past a ray's termination are evaluated and discarded, like the
-	// reference's own n_steps > 1 batching; frames are bit-identical with or without helpers. help_mode 1: only once the queue is exhausted, 2: always.
-	// Compiled only into the experiment build (NSB_X_HELP=1); not measured on the H100.
-	const bool fx_show_accel = NSB_X_ACCEL && f.show_accel;
-	const int fx_glow = NSB_X_GLOW ? f.glow_mode : 0;
-	const float* const fx_ray_od = NSB_X_RAYOD ? ray_od : nullptr;
-	const int help_mode = (!NSB_X_HELP || OPS || (fx_glow & 4)) ? 0 : (dda_flags >> 16) & 3;  // host: NSB_HELPERS (the mailbox does not carry glow's weight mask)
-	constexpr uint32_t HELP_DEPTH = 7;
-	// mailbox helper -> owner: the tile's operand space is idle between the end of run_network (which ends on a tile barrier) and the next
-	// encode, and every warp only ever writes its own 512 bytes of each k-chunk: field q of lane l lives in k-chunk q
-	float* const mbox = reinterpret_cast<float*>(TB.a64 + (tid >> 5) * 512u) + lane;
-	constexpr uint32_t MB = tc::ROWS * 16 / 4;  // floats between mailbox fields
-	enum { M_ALPHA = 0, M_E0, M_E1, M_E2, M_Z, M_TNEXT };  // M_TNEXT < 0: not a sample
 	constexpr bool ops_on = OPS;  // the host picks the instantiation: f.apply_ops && n_ops > 0
 
 	// what stays in registers across a round
 	bool alive = false, exhausted = false;  // exhausted is warp-uniform: the queue had nothing left when this warp last asked
-	uint32_t ch_next = 0, ch_end = 0;       // this warp's chunk of the ray queue (warp-uniform)
 	uint32_t pix = 0, n_steps = 0;
 	uint32_t c_hit = 0, c_samples = 0, c_old = 0;
 	// phase profile (thread 0 of each CTA; a handful of clock reads per round): diagnostic builds only (-DNSB_PROFILE), the
@@ -299,45 +252,29 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 		bool has_sample = false;
 		float dt = 0.0f;
 		V3 pos = v3(0, 0, 0), dw = v3(0.5f, 0.5f, 0.5f);
-		int h_owner = -1;                  // >= 0: this lane helps the ray of that lane this round
-		float h_tnext = -1.0f;             // helper: t after its sample
-		unsigned h_free = 0u;              // warp-uniform: the helper lanes of this round (0: none)
-		uint32_t h_per_ray = 0, h_first = 0;  // owner: its helpers are the h_per_ray free lanes from free-rank h_first
 		{
-			int budget = dda_budget;
+			int budget = DDA_BUDGET;
 			V3 ro = v3(TB.ray[R_OX][tid], TB.ray[R_OY][tid], TB.ray[R_OZ][tid]);
 			V3 rd = v3(TB.ray[R_DX][tid], TB.ray[R_DY][tid], TB.ray[R_DZ][tid]);
 			float t = TB.ray[R_T][tid];
-			// Refill (warp-convergent). Free lanes wait until the warp is down to <= refill_thr live rays; rays come from a queue CHUNK
-			// this warp owns (consecutive entries = neighbouring pixels), so the lanes of a warp gather from the same few hash-grid
-			// cells on the coarse and middle levels instead of 32 unrelated cache lines per instruction.
+			// Refill (warp-convergent). Free lanes wait until the warp is down to <= REFILL_THR live rays, then take consecutive queue
+			// entries (neighbouring pixels) in one claim, so the lanes of a warp gather from the same few hash-grid cells on the coarse
+			// and middle levels instead of 32 unrelated cache lines per instruction.
 			{
 				const unsigned alive_m = __ballot_sync(0xffffffffu, alive);
 				const unsigned want = exhausted ? 0u : ~alive_m;
-				if (want && __popc(alive_m) <= (refill_thr & 0xff)) {
+				if (want && __popc(alive_m) <= REFILL_THR) {
 					const uint32_t need = (uint32_t)__popc(want), rank = (uint32_t)__popc(want & ((1u << lane) - 1u));
-					const uint32_t chunk = (uint32_t)refill_thr >> 8;
-					uint32_t given = 0, qi = 0xffffffffu;
-					while (given < need) {  // warp-uniform
-						if (ch_next >= ch_end) {
-							const uint32_t claim = chunk ? chunk : need - given;
-							uint32_t base = 0;
-							if (lane == 0) base = atomicAdd(fetch_counter, claim);
-							base = __shfl_sync(0xffffffffu, base, 0);
-							if (base >= n_queued) { exhausted = true; break; }
-							ch_next = base;
-							ch_end = min(base + claim, n_queued);
-						}
-						const uint32_t take = min(need - given, ch_end - ch_next);
-						if (!alive && rank >= given && rank < given + take) qi = ch_next + (rank - given);
-						ch_next += take;
-						given += take;
-					}
-					if (qi != 0xffffffffu) {
+					uint32_t base = 0;
+					if (lane == 0) base = atomicAdd(fetch_counter, need);
+					base = __shfl_sync(0xffffffffu, base, 0);
+					exhausted = base + need > n_queued;  // a short claim: the queue has nothing left for this warp
+					const uint32_t qi = base + rank;     // free lane of free-rank `rank`
+					if (!alive && qi < n_queued) {
 						const RayRec rr = list[qi];
 						pix = rr.pix;
-						if (fx_ray_od) {  // a general-camera frame: k_prepare_rays<true> left the ray next to its queue entry
-							const float* od = fx_ray_od + 6 * (size_t)qi;
+						if (ray_od) {  // a general-camera frame: k_prepare_rays<true> left the ray next to its queue entry
+							const float* od = ray_od + 6 * (size_t)qi;
 							ro = v3(od[0], od[1], od[2]); rd = v3(od[3], od[4], od[5]);
 						} else {
 							Ray r;
@@ -371,43 +308,6 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 				t = add(t, dt);
 			}
 			if (alive) TB.ray[R_T][tid] = t;
-			if constexpr (!OPS) {
-				if (help_mode == 2 || (help_mode == 1 && exhausted)) {
-					const unsigned smp_m = __ballot_sync(0xffffffffu, has_sample);  // rays that found a sample this round
-					const unsigned free_m = ~__ballot_sync(0xffffffffu, alive);     // lanes without a ray
-					const uint32_t n_smp = (uint32_t)__popc(smp_m), n_free = (uint32_t)__popc(free_m);
-					if (n_smp != 0u && n_free != 0u) {
-						h_free = free_m;
-						h_per_ray = n_free >= n_smp ? min(HELP_DEPTH, n_free / n_smp) : 1u;  // fewer free lanes than rays: the first n_free rays get one each
-						uint32_t depth = 0;
-						if (!alive) {
-							const uint32_t q = (uint32_t)__popc(free_m & ((1u << lane) - 1u));
-							const uint32_t k = q / h_per_ray;
-							if (k < n_smp) { h_owner = (int)nth_set_bit(smp_m, k); depth = 1u + q % h_per_ray; }
-						} else if (has_sample) {
-							h_first = (uint32_t)__popc(smp_m & ((1u << lane) - 1u)) * h_per_ray;
-							if (h_first >= n_free) h_per_ray = 0;
-						}
-						const int sl = h_owner < 0 ? (int)lane : h_owner;
-						const V3 hro = v3(__shfl_sync(0xffffffffu, ro.x, sl), __shfl_sync(0xffffffffu, ro.y, sl), __shfl_sync(0xffffffffu, ro.z, sl));
-						const V3 hrd = v3(__shfl_sync(0xffffffffu, rd.x, sl), __shfl_sync(0xffffffffu, rd.y, sl), __shfl_sync(0xffffffffu, rd.z, sl));
-						float tj = __shfl_sync(0xffffffffu, t, sl);                  // the owner's t after its own sample
-						const uint32_t hsteps = __shfl_sync(0xffffffffu, n_steps, sl);  // ... and its step count before it
-						if (h_owner >= 0) {
-							for (uint32_t i = 1; i < depth; ++i) tj = add(tj, calc_dt(tj, f.cone));  // the march of :671-688 over occupied samples
-							pos = madd3(hrd, tj, hro);
-							bool ok = hsteps + depth < MARCH_ITER - 1 && box_contains(f.rmin, f.rmax, pos);
-							dt = calc_dt(tj, f.cone);
-							if (ok && bitfield) {
-								const uint32_t mip = (uint32_t)max(f.min_mip, mip_from_dt(dt, pos));
-								ok = bitfield_at(cascaded_grid_idx_at(pos, mip), mip, bitfield);
-							}
-							has_sample = ok;
-							if (ok) { dw = warp_direction(hrd); h_tnext = add(tj, dt); }
-						}
-					}
-				}
-			}
 		}
 
 		// ---- network inputs: generate_next_nerf_network_inputs :690 ----
@@ -421,7 +321,8 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 		if (has_sample) {
 			pw = warp_position(pos, f.tmin, f.tmax);
 			dtw = warp_dt(dt);
-			if (h_owner < 0) { ++n_steps; ++c_samples; }  // a helper's sample is counted by the owner when it composites it
+			++n_steps;
+			++c_samples;
 			if (ops_on) {
 				if (any_poisson) {  // membrane residuals are evaluated in deformed space (:2867-2883)
 					poisson_one(ops, n_ops, pw, mem);
@@ -464,11 +365,10 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 		const long long c3 = clock64();
 #endif
 
-		// ---- composite_kernel_nerf :750-955, split in two: what depends on the sample alone (any lane), then the ray's running sums (its owner lane) ----
+		// ---- composite_kernel_nerf :750-955, split in two: what depends on the sample alone, then the ray's running sums ----
 		float s_alpha = 0.0f, s_e[3] = {0.0f, 0.0f, 0.0f}, s_z = 0.0f;
 		float s_mask = 1.0f;  // glow_mode's mask_to_alpha: multiplies the sample's weight (:877-879)
 		if (has_sample) {
-			const uint32_t rtid = h_owner < 0 ? tid : (tid & ~31u) + (uint32_t)h_owner;  // the slot of the ray this sample belongs to
 			const V3 cam_fwd = v3(f.cam1[6], f.cam1[7], f.cam1[8]);
 			V3 cpos = unwarp_position(pw, f.tmin, f.tmax);
 			float dtu = unwarp_dt(dtw);
@@ -489,16 +389,16 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 			} else {
 				alpha = 1.0f - __expf(-sigma * dtu);
 			}
-			if (fx_show_accel) alpha = 1.0f;  // show_accel >= 0: the occupancy cells themselves are drawn (:788-790)
+			if (f.show_accel) alpha = 1.0f;  // show_accel >= 0: the occupancy cells themselves are drawn (:788-790)
 			float rgb[3] = {network_to_rgb(h_lo(rgbo[0]), f.rgb_act), network_to_rgb(h_hi(rgbo[0]), f.rgb_act), network_to_rgb(h_lo(rgbo[1]), f.rgb_act)};
-			if (fx_glow) {  // :807-903, before the mode overrides
-				const float4 gl = glow_apply(fx_glow, f.glow_y_cutoff, cpos, v3(f.cam1[9], f.cam1[10], f.cam1[11]), rgb[0], rgb[1], rgb[2]);
+			if (f.glow_mode) {  // :807-903, before the mode overrides
+				const float4 gl = glow_apply(f.glow_mode, f.glow_y_cutoff, cpos, v3(f.cam1[9], f.cam1[10], f.cam1[11]), rgb[0], rgb[1], rgb[2]);
 				rgb[0] = gl.x; rgb[1] = gl.y; rgb[2] = gl.z; s_mask = gl.w;
 			}
 			if (f.mode != NSB_RENDER_SHADE) {
-				const V3 ro = v3(TB.ray[R_OX][rtid], TB.ray[R_OY][rtid], TB.ray[R_OZ][rtid]);
+				const V3 ro = v3(TB.ray[R_OX][tid], TB.ray[R_OY][tid], TB.ray[R_OZ][tid]);
 				if (f.mode == NSB_RENDER_AO) { rgb[0] = rgb[1] = rgb[2] = alpha; }
-				else if (f.mode == NSB_RENDER_POSITIONS && fx_show_accel) {  // one random colour per occupancy cell (:913-923)
+				else if (f.mode == NSB_RENDER_POSITIONS && f.show_accel) {  // one random colour per occupancy cell (:913-923)
 					const uint32_t mip = (uint32_t)max(f.min_mip, mip_from_pos(cpos));
 					const float res = (float)(GRIDSIZE >> mip);
 					const int ix = (int)mul(cpos.x, res), iy = (int)mul(cpos.y, res), iz = (int)mul(cpos.z, res);
@@ -529,16 +429,7 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 			s_alpha = alpha; s_e[0] = rgb[0]; s_e[1] = rgb[1]; s_e[2] = rgb[2];
 			s_z = dot3(cam_fwd, vsub(cpos, v3(f.cam1[9], f.cam1[10], f.cam1[11])));
 		}
-		if constexpr (!OPS) {
-			if (h_free) {  // warp-uniform: helpers post their samples, owners read them below
-				if (h_owner >= 0) {
-					mbox[M_TNEXT * MB] = h_tnext;
-					if (has_sample) { mbox[M_ALPHA * MB] = s_alpha; mbox[M_E0 * MB] = s_e[0]; mbox[M_E1 * MB] = s_e[1]; mbox[M_E2 * MB] = s_e[2]; mbox[M_Z * MB] = s_z; }
-				}
-				__syncwarp();
-			}
-		}
-		if (has_sample && h_owner < 0) {
+		if (has_sample) {
 			const float sat = 1.0f - f.min_T;  // rendering_min_transmittance test of composite_kernel_nerf :951
 			float cr = TB.ray[R_CR][tid], cg = TB.ray[R_CG][tid], cb = TB.ray[R_CB][tid], ca = TB.ray[R_CA][tid];
 			float ray_depth = TB.ray[R_DEPTH][tid], max_weight = TB.ray[R_MAXW][tid];
@@ -559,7 +450,7 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 					finish(false, cr, cg, cb, ca, ray_depth);
 				}
 			};
-			if (fx_glow & 4) {
+			if (f.glow_mode & 4) {
 				// mask_to_alpha: weight *= mask (a separate copy so that the unmasked expression — and its FMA contraction — stays exactly the reference's)
 				float T = 1.0f - ca;
 				float weight = s_alpha * T;
@@ -576,22 +467,6 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 				}
 			} else {
 				accumulate(s_alpha, s_e[0], s_e[1], s_e[2], s_z);
-			}
-			if constexpr (!OPS) {
-				if (h_free && h_per_ray) {  // this ray's helpers: consecutive free lanes from free-rank h_first, in march order
-					const float* wbox = mbox - lane;
-					uint32_t hl = nth_set_bit(h_free, h_first);
-					const uint32_t n_free = (uint32_t)__popc(h_free);
-					for (uint32_t i = 0; alive && i < h_per_ray && h_first + i < n_free; ++i) {
-						const float tn = wbox[M_TNEXT * MB + hl];
-						if (tn < 0.0f) break;  // not an occupied in-bounds sample: the march resumes there next round
-						++n_steps;
-						++c_samples;
-						accumulate(wbox[M_ALPHA * MB + hl], wbox[M_E0 * MB + hl], wbox[M_E1 * MB + hl], wbox[M_E2 * MB + hl], wbox[M_Z * MB + hl]);
-						TB.ray[R_T][tid] = tn;
-						hl = (uint32_t)__ffs((int)(h_free & ~((2u << hl) - 1u))) - 1u;  // next free lane
-					}
-				}
 			}
 			if (alive) {
 				TB.ray[R_CR][tid] = cr; TB.ray[R_CG][tid] = cg; TB.ray[R_CB][tid] = cb; TB.ray[R_CA][tid] = ca;
@@ -626,8 +501,6 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 		if (lane == 0 && v) atomicAdd(stats + slot[k], v);
 	}
 }
-
-#include "nsb_render_ws.cuh"
 
 // =====================================================================================================
 // operator-level kernels (same device code as the fused renderer)
@@ -1057,7 +930,6 @@ static NsbStatus fail(NsbStatus s, const char* fmt, ...) {
 struct NsbContext {
 	int device = 0;
 	int sm_count = 0;
-	int ctas_per_sm = 1;
 	int inference_ctas_per_sm = 1;
 	int grid_update_ctas_per_sm = 1;
 	bool has_model = false, has_occ = false;
@@ -1094,10 +966,6 @@ struct NsbContext {
 	float* d_ray_od = nullptr;     // origin + direction per queue slot, general-camera frames only (allocated on the first such frame)
 	size_t ray_od_capacity = 0;
 	int acc16 = 1;                 // MLP accumulator policy: 1 fp16 wgmma accumulators (default: the reference's wmma __half fragments), 0 fp32 (nsb_set_mlp_accumulator)
-	int use_ws = 0;                // NSB_WS=1: frames without operators go through the warp-specialised kernel (experimental; default k_render_fused<false>)
-	int helpers = 0;               // helper lanes of k_render_fused (experiment build only, -DNSB_X_HELP=1): 0 off (default), 1 once the queue is exhausted, 2 always (NSB_HELPERS)
-	int refill_thr = 2;            // lanes of a warp refill when at most this many of its rays are alive (31: immediately)
-	int dda_budget = DDA_BUDGET;
 	cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr;  // start, end, between k_prepare_rays and k_render_fused
 	bool timed = false;
 	uint32_t launches = 0;
@@ -1192,9 +1060,8 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 		if (pct > 100) pct = 100;
 		return cudaFuncSetAttribute(func, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
 	};
-	// k_render_fused: ONE CTA of NSB_TILES (NSB_TILES_OPS with operators) tiles per SM (768 x 80 / 640 x 96 registers = the register file;
+	// k_render_fused: ONE CTA of RENDER_TILES (RENDER_TILES_OPS with operators) tiles per SM (768 x 80 / 640 x 96 registers = the register file;
 	// shared memory 20 KB weights + 22.5 KB per tile).
-	c->ctas_per_sm = 1;
 	CU(set_smem((const void*)k_render_fused<false, false>, sizeof(RenderSmemT<render_tiles(false)>), 1));
 	CU(set_smem((const void*)k_render_fused<true, false>, sizeof(RenderSmemT<render_tiles(true)>), 1));
 	CU(set_smem((const void*)k_render_fused<false, true>, sizeof(RenderSmemT<render_tiles(false)>), 1));
@@ -1221,17 +1088,6 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 		CU(set_smem((const void*)k_density_grid_update<false>, sizeof(tc::TileSmem), c->grid_update_ctas_per_sm));
 		CU(set_smem((const void*)k_density_grid_update<true>, sizeof(tc::TileSmem), c->grid_update_ctas_per_sm));
 	}
-	if (const char* e = getenv("NSB_CARVEOUT")) {  // experiments
-		CU(cudaFuncSetAttribute(k_render_fused<false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(e)));
-		CU(cudaFuncSetAttribute(k_render_fused<true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(e)));
-	}
-	CU(set_smem((const void*)k_render_ws, sizeof(ws::Smem), 1));
-	if (const char* e = getenv("NSB_WS")) c->use_ws = atoi(e) != 0;
-	if (const char* e = getenv("NSB_MLP_ACC16")) c->acc16 = atoi(e) != 0;
-	if (const char* e = getenv("NSB_REFILL_THR")) { int v = atoi(e); if (v >= 0 && v <= 31) c->refill_thr = v; }
-	if (const char* e = getenv("NSB_HELPERS")) { int v = atoi(e); if (v >= 0 && v <= 2) c->helpers = v; }
-	if (const char* e = getenv("NSB_CHUNK")) { int v = atoi(e); if (v >= 0 && v <= 65535) c->refill_thr |= v << 8; }
-	if (const char* e = getenv("NSB_DDA_BUDGET")) { int v = atoi(e); if (v >= 0 && v <= 1024) c->dda_budget = v; }
 	if (getenv("NSB_VERBOSE"))
 		fprintf(stderr, "[nsb] device %d: %d SMs; k_render_fused %d tiles/CTA (%d with operators), %d regs, %zu B smem; inference %d CTAs/SM, grid update %d CTAs/SM\n", device, c->sm_count,
 		        render_tiles(false), render_tiles(true), fa.numRegs, sizeof(RenderSmemT<render_tiles(false)>), c->inference_ctas_per_sm, c->grid_update_ctas_per_sm);
@@ -1885,19 +1741,11 @@ extern "C" NsbStatus nsb_render(NsbContext* c, const NsbFrame* frame, float* fb_
 		CU(cudaEventRecord(c->evm, stream));
 		const bool ops_on = f.apply_ops && c->n_ops > 0;
 		const uint32_t tiles = (uint32_t)render_tiles(ops_on);
-		uint32_t grid = (uint32_t)(c->sm_count * c->ctas_per_sm);
+		uint32_t grid = (uint32_t)c->sm_count;  // one CTA per SM
 		if (grid > (my_tiles + tiles - 1) / tiles) grid = (my_tiles + tiles - 1) / tiles;
-		if (!ops_on && c->use_ws && !c->acc16 && !f.show_accel && !f.general_camera && !f.glow_mode && (uint64_t)f.W * (uint64_t)f.H < (1ull << 28)) {  // k_render_ws ships the pixel in 28 bits of a flag word
-			uint32_t g2 = (uint32_t)c->sm_count;
-			if (g2 > (my_tiles + ws::PT - 1) / ws::PT) g2 = (uint32_t)((my_tiles + ws::PT - 1) / ws::PT);
-			k_render_ws<<<g2, ws::THREADS, sizeof(ws::Smem), stream>>>(f, c->model, c->has_occ ? c->d_bitfield : nullptr, reinterpret_cast<float4*>(fb_dev), depth_dev, c->d_list,
-			                                                           c->d_counters, c->d_counters + 1, c->d_stats, c->refill_thr, c->dda_budget);
-		} else {
 		auto kernel = ops_on ? (c->acc16 ? k_render_fused<true, true> : k_render_fused<true, false>) : (c->acc16 ? k_render_fused<false, true> : k_render_fused<false, false>);
 		kernel<<<grid, 128 * tiles, ops_on ? sizeof(RenderSmemT<render_tiles(true)>) : sizeof(RenderSmemT<render_tiles(false)>), stream>>>(f, c->model, c->has_occ ? c->d_bitfield : nullptr, c->d_ops, c->n_ops, c->any_poisson,
-		                                                          reinterpret_cast<float4*>(fb_dev), depth_dev, c->d_list, ray_od, c->d_counters, c->d_counters + 1, c->d_stats,
-		                                                          c->refill_thr, c->dda_budget | (c->helpers << 16));
-		}
+		                                                          reinterpret_cast<float4*>(fb_dev), depth_dev, c->d_list, ray_od, c->d_counters, c->d_counters + 1, c->d_stats);
 		CU(cudaGetLastError());
 	}
 	CU(cudaEventRecord(c->ev1, stream));

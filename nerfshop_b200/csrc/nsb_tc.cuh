@@ -57,9 +57,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 	asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-	asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -80,29 +77,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 			long long now = clock64();
 			if (t0 == 0) t0 = now;
 			else if (now - t0 > 4000000000ll) __trap();
-		}
-	}
-}
-// The same wait for a barrier whose completion is thousands of cycles away (the warp-specialised renderer's producer <-> consumer hand-offs):
-// a spinning warp takes issue slots from the warps it is waiting for, so back off with nanosleep between polls.
-__device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity, uint32_t ns) {
-	uint32_t addr = smem_u32(bar);
-	uint32_t done = 0;
-	long long t0 = 0;
-	for (uint32_t spins = 0;; ++spins) {
-		asm volatile(
-			"{\n\t.reg .pred p;\n\t"
-			"mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-			"selp.u32 %0, 1, 0, p;\n\t}"
-			: "=r"(done)
-			: "r"(addr), "r"(parity)
-			: "memory");
-		if (done) break;
-		__nanosleep(ns);
-		if ((spins & 4095u) == 4095u) {
-			long long now = clock64();
-			if (t0 == 0) t0 = now;
-			else if (now - t0 > 8000000000ll) __trap();
 		}
 	}
 }
@@ -299,24 +273,19 @@ __device__ __forceinline__ void store_out16(uint8_t* base, uint32_t chunk, uint3
 //   density_only: stop after L2 (NerfNetwork::density)
 //   dens[8]: the 16 fp16 outputs of the density MLP (packed half2), rgb[8]: the 16 outputs of the rgb MLP, both for sample c.row.
 // `dw` = this sample's warped view direction; its 16 SH values are evaluated between L2 and L3.
-// `a_first`: shared-window address of the first layer's operand when it does not live in c.a32 (the warp-specialised renderer's producers
-// write the grid features into their own operand); 0 = c.a32. `release`: an mbarrier to arrive on (one arrival) once every warp's first
-// layer has read that operand.
 // Operand space: chunks 0-3 the 32-wide layer inputs, 4-5 the rgb hand-back, 6-7 the density hand-back. On return the whole tile has
 // finished with the operand space, so the caller may overwrite any of it.
 template <bool ACC16 = false>
-__device__ __forceinline__ void run_network(const TileCtx& c, V3 dw, bool density_only, uint32_t* dens, uint32_t* rgb, uint32_t a_first = 0,
-                                            uint64_t* release = nullptr) {
+__device__ __forceinline__ void run_network(const TileCtx& c, V3 dw, bool density_only, uint32_t* dens, uint32_t* rgb) {
 	const uint32_t row = c.row;
 	const uint32_t a32 = smem_u32(c.a32), w = c.w_addr;
-	if (a_first == 0) a_first = a32;
 	fence_async_smem();
 	tile_sync(c);  // every sample's grid features are in place
 #pragma unroll 1
 	for (uint32_t h = 0; h < 2; ++h) {
 		Acc<64, ACC16> x;
 		Acc<16, ACC16> o;
-		layer_ss<64, 32, ACC16>(x.r, a_first + h * 64 * 16, w + W1_OFF);  // L1: grid features (32) -> 64
+		layer_ss<64, 32, ACC16>(x.r, a32 + h * 64 * 16, w + W1_OFF);      // L1: grid features (32) -> 64
 		layer_rs<16, 64, ACC16>(o.r, x.r, w + W2_OFF);                    // L2: 64 -> 16
 		store_out16<ACC16>(c.a32, 6, row, h, o.r);
 	}
@@ -327,7 +296,6 @@ __device__ __forceinline__ void run_network(const TileCtx& c, V3 dw, bool densit
 	}
 	tile_sync(c);  // every warp's first layer has read its operand
 	if (density_only) return;
-	if (release && row == 0) mbar_arrive(release);
 	// rgb-network input: columns 0-15 = density MLP output, 16-31 = SH (nerf_network_full.h:52,67,79)
 	__half2 sh[8];
 	encode_sh4(dw, sh);  // tcnn SphericalHarmonics of the (mapped) direction

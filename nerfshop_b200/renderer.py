@@ -24,12 +24,11 @@ def _torch():
 
 
 class NerfRenderer:
-    def __init__(self, device: int | None = None, lib_path: str | None = None):
-        """lib_path: an experiment build of the same library (nerfshop_b200.build.build_variant); default = the product library."""
+    def __init__(self, device: int | None = None):
         torch = _torch()
         if not torch.cuda.is_available():
             raise abi.NsbError("no CUDA device: nerfshop_b200 has no CPU fallback")
-        self.lib = abi.load_library(lib_path)
+        self.lib = abi.load_library()
         self.device = torch.cuda.current_device() if device is None else device
         self.ctx = C.c_void_p()
         abi.check(self.lib, self.lib.nsb_create(self.device, C.byref(self.ctx)), "nsb_create")

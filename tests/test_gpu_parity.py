@@ -227,47 +227,6 @@ def test_full_size_properties(scene, renderer):
     assert st1.n_samples > 20 * st1.n_hit * 0.2
 
 
-def test_helper_lanes_do_not_change_the_frame(scene, monkeypatch):
-    """k_render_fused lends the lanes without a ray to the rays that have one (up to 7 further samples per ray and round, composited in march
-    order by the ray's own lane; NSB_HELPERS in the experiment build -DNSB_X_HELP=1). Scheduling only: frames, depth and the ray / sample / hit counts are bit-identical
-    with helpers off (0, the default), in the frame's tail only (1) and always (2) — at 1080p, at a ragged size, on a tile partition and in every render mode."""
-    import torch
-
-    from nerfshop_b200 import build
-    from nerfshop_b200.renderer import NerfRenderer
-
-    # the helper-lane code is compiled out of the product (its presence alone costs 5 %): this is the experiment build of the same sources
-    helpers_lib = os.path.join(build.LIB_DIR, "libnerfshop_b200_helpers.so")
-    if not os.path.exists(helpers_lib) or os.path.getmtime(helpers_lib) < os.path.getmtime(build.build()):
-        build.build_variant("helpers", ["NSB_X_HELP=1"])
-    model, occ = scene
-    cams = syn.orbit_cameras(120)
-    jobs = [(syn.make_frame(model, cams[17], 1920, 1080), "1080p"), (syn.make_frame(model, cams[44], 333, 187), "ragged"),
-            (syn.make_frame(model, cams[80], 640, 360, rank=3, world=8), "partition")]
-    for mode in (abi.NSB_RENDER_AO, abi.NSB_RENDER_POSITIONS, abi.NSB_RENDER_DEPTH, abi.NSB_RENDER_STEPSIZE, abi.NSB_RENDER_COST):
-        f = syn.make_frame(model, cams[5], 480, 270)
-        f.mode = mode
-        jobs.append((f, f"mode {mode}"))
-    results = {}
-    for helpers in ("0", "1", "2"):
-        monkeypatch.setenv("NSB_HELPERS", helpers)
-        r = NerfRenderer(0, lib_path=helpers_lib)
-        r.upload_model(model.desc, model.params)
-        r.upload_occupancy(occ)
-        out = []
-        for f, _ in jobs:
-            fb, d = r.render(f)
-            st = r.stats()
-            out.append((fb.clone(), d.clone(), (st.n_rays, st.n_samples, st.n_hit)))
-        torch.cuda.synchronize()
-        results[helpers] = out
-        r.close()
-    for helpers in ("1", "2"):
-        for (fb0, d0, st0), (fb, d, st), (_, name) in zip(results["0"], results[helpers], jobs):
-            assert st == st0, (helpers, name, st, st0)
-            assert torch.equal(fb, fb0) and torch.equal(d, d0), (helpers, name)
-
-
 def test_async_host_frames_equal_the_synchronous_ones(scene, renderer):
     """nsb_render_host_async / nsb_host_frame_wait: five frames through two slots in flight equal nsb_render_host's, tickets count up, and a bad
     ticket is an error."""

@@ -1,6 +1,6 @@
-"""A/B timing of library variants / environment knobs on the 1080p orbit (4 cameras, L2 flushed, CUDA events inside nsb_render).
+"""A/B timing of library builds on the 1080p orbit (4 cameras, L2 flushed, CUDA events inside nsb_render).
 
-  python tools/ab_kernels.py name=LIBPATH[,ENV=VAL,...] ...        e.g.  base=,NSB_WS=0  ws=,NSB_WS=1  prof=nerfshop_b200/lib/libnerfshop_b200_prof.so
+  python tools/ab_kernels.py name=LIBPATH ...        e.g.  base=  prof=nerfshop_b200/lib/libnerfshop_b200_prof.so   (empty LIBPATH: the product library)
 Each variant runs in its own process (the library is loaded once per process). Prints fused-kernel ms (mean over the cameras), samples, debug counters
 and a checksum of frame 0 (variants that must be bit-identical can be compared)."""
 import json
@@ -52,16 +52,10 @@ if len(sys.argv) > 1 and sys.argv[1] == "--child":
     sys.exit(0)
 
 for spec in sys.argv[1:]:
-    name, rest = spec.split("=", 1)
-    parts = rest.split(",")
+    name, path = spec.split("=", 1)
     env = dict(os.environ)
-    if parts[0]:
-        env["NSB_LIB_PATH"] = os.path.join(ROOT, parts[0]) if not os.path.isabs(parts[0]) else parts[0]
-    for kv in parts[1:]:
-        if not kv:
-            continue
-        k, v = kv.split("=")
-        env[k] = v
+    if path:
+        env["NSB_LIB_PATH"] = os.path.join(ROOT, path)
     res = subprocess.run([sys.executable, os.path.abspath(__file__), "--child"], env=env, capture_output=True, text=True, timeout=600)
     line = res.stdout.strip().splitlines()[-1] if res.stdout.strip() else "FAILED: " + res.stderr[-400:]
     print(f"{name:16s} {line}", flush=True)
