@@ -30,7 +30,7 @@ struct DevLevel {
 	uint32_t size;    // entries (2 x fp16 each)
 	uint32_t res2;    // res*res (0 for hashed levels)
 	uint32_t hashed;  // 1: spatial hash, 0: dense
-	uint32_t mask;    // size-1 when size is a power of two, else 0
+	uint32_t mask;    // size-1 of a hashed level (a power of two, see build_levels); 0 for dense levels
 	const __half2* base;  // first entry of the level (table + level offset): one IMAD.WIDE per gather address
 };
 
@@ -546,7 +546,7 @@ __device__ __forceinline__ uint32_t grid_index(const DevLevel& L, uint32_t gx, u
 	uint32_t h = 0, d = 0;
 	if (MODE != 0) {
 		h = gx ^ (gy * 2654435761u) ^ (gz * 805459861u);
-		h = L.mask ? (h & L.mask) : (h % L.size);
+		h &= L.mask;  // tcnn's `index % size`: a hashed level's size is a power of two (build_levels)
 	}
 	if (MODE != 1) {
 		d = gx + gy * L.res + gz * L.res2;

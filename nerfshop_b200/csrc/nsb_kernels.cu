@@ -1004,7 +1004,9 @@ static bool build_levels(const NsbModelDesc* d, DevLevel* L, uint64_t* n_grid_en
 		L[l].size = n;
 		L[l].hashed = dense > (double)n ? 1u : 0u;
 		L[l].res2 = L[l].hashed ? 0u : res * res;
-		L[l].mask = (n & (n - 1)) == 0 ? n - 1 : 0u;
+		// Hashed implies size = 2^log2_hashmap_size: n is res^3 rounded up to a multiple of 8 (>= res^3: dense) or the table cap.
+		// So mask = size - 1, and grid_index takes a hashed level's `index % size` as `index & mask`.
+		L[l].mask = L[l].hashed ? n - 1 : 0u;
 		offset += n;
 	}
 	*n_grid_entries = offset;
