@@ -50,6 +50,8 @@ struct DevFrame {
 	float rs[4];
 	float rmin[3], rmax[3];  // render aabb
 	float tmin[3], tmax[3];  // train aabb
+	float tinv[3];           // per axis: 1 / (tmax - tmin) when that extent is a power of two (exact), else 0
+	int tinv_exact;          // all three tinv are set: warp_position may multiply instead of divide
 	float cone, min_T, depth_scale;
 	int rgb_act, density_act, mode;
 	uint32_t spp;
@@ -187,6 +189,11 @@ __device__ __forceinline__ float box_ray_tmin(const float* mn, const float* mx, 
 __device__ __forceinline__ V3 warp_position(V3 p, const float* mn, const float* mx) {
 	return v3(div_(sub(p.x, mn[0]), sub(mx[0], mn[0])), div_(sub(p.y, mn[1]), sub(mx[1], mn[1])), div_(sub(p.z, mn[2]), sub(mx[2], mn[2])));
 }
+// warp_position for extents 2^k with the exact inverses 2^-k: (p - mn) / 2^k and (p - mn) * 2^-k are both the correctly rounded value of
+// the same real number, subnormals included
+__device__ __forceinline__ V3 warp_position_pow2(V3 p, const float* mn, const float* inv) {
+	return v3(mul(sub(p.x, mn[0]), inv[0]), mul(sub(p.y, mn[1]), inv[1]), mul(sub(p.z, mn[2]), inv[2]));
+}
 __device__ __forceinline__ V3 unwarp_position(V3 p, const float* mn, const float* mx) {
 	return v3(fma_(p.x, sub(mx[0], mn[0]), mn[0]), fma_(p.y, sub(mx[1], mn[1]), mn[1]), fma_(p.z, sub(mx[2], mn[2]), mn[2]));
 }
@@ -194,20 +201,25 @@ __device__ __forceinline__ V3 warp_direction(V3 d) { return v3(mul(add(d.x, 1.0f
 __device__ __forceinline__ V3 unwarp_direction(V3 d) { return v3(fma_(d.x, 2.0f, -1.0f), fma_(d.y, 2.0f, -1.0f), fma_(d.z, 2.0f, -1.0f)); }
 __device__ __forceinline__ float warp_dt(float dt) { return div_(sub(dt, MIN_STEP()), DT_RANGE()); }
 __device__ __forceinline__ float unwarp_dt(float dt) { return fma_(dt, DT_RANGE(), MIN_STEP()); }
-__device__ __forceinline__ float calc_dt(float t, float cone) { return clampf(mul(t, cone), MIN_STEP(), MAX_STEP()); }
+// t·cone is never NaN (t and cone are finite), and on non-NaN input clamp(x, lo, hi) == min(max(x, lo), hi): two FMNMX
+__device__ __forceinline__ float calc_dt(float t, float cone) { return fminf(fmaxf(mul(t, cone), MIN_STEP()), MAX_STEP()); }
 
-__device__ __forceinline__ float distance_to_next_voxel(V3 pos, V3 dir, V3 idir, uint32_t res) {  // :93-101
-	float fr = (float)res;  // 128 >> mip: a power of two, so t / fr == t * (1 / fr) bit for bit
+// floor(fma(0.5, copysign(1, d), p + 0.5)) is not floor(p) + (d >= 0): p + 0.5 rounds when it crosses a binade (p = 1 - 2^-24 gives 1.5,
+// then 2), so the reference's expression is kept as it is
+__device__ __forceinline__ float distance_to_next_voxel(V3 pos, V3 dir, V3 idir, uint32_t mip) {  // :93-101
+	float fr = __uint_as_float((134u - mip) << 23);  // the cascade's resolution 128 >> mip = 2^(7 - mip), exact
 	float px = mul(fr, pos.x), py = mul(fr, pos.y), pz = mul(fr, pos.z);
 	float tx = mul(sub(floorf(fma_(0.5f, copysignf(1.0f, dir.x), add(px, 0.5f))), px), idir.x);
 	float ty = mul(sub(floorf(fma_(0.5f, copysignf(1.0f, dir.y), add(py, 0.5f))), py), idir.y);
 	float tz = mul(sub(floorf(fma_(0.5f, copysignf(1.0f, dir.z), add(pz, 0.5f))), pz), idir.z);
 	float t = fminf(fminf(tx, ty), tz);
-	return fmaxf(mul(t, __uint_as_float(0x7f000000u - __float_as_uint(fr))), 0.0f);
+	return fmaxf(mul(t, __uint_as_float((120u + mip) << 23)), 0.0f);  // fr is a power of two, so t / fr == t * 2^(mip - 7) bit for bit
 }
-__device__ __forceinline__ float advance_to_next_voxel(float t, float cone, V3 pos, V3 dir, V3 idir, uint32_t res) {  // :103-115
-	float t_target = add(t, distance_to_next_voxel(pos, dir, idir, res));
-	do { t = add(t, calc_dt(t, cone)); } while (t < t_target);
+// dt: calc_dt(t, cone), which the caller already has; the reference's do-while computes it again in its first iteration
+__device__ __forceinline__ float advance_to_next_voxel(float t, float dt, float cone, V3 pos, V3 dir, V3 idir, uint32_t mip) {  // :103-115
+	float t_target = add(t, distance_to_next_voxel(pos, dir, idir, mip));
+	t = add(t, dt);
+	while (t < t_target) t = add(t, calc_dt(t, cone));
 	return t;
 }
 __host__ __device__ __forceinline__ uint32_t expand_bits(uint32_t v) {
@@ -218,35 +230,54 @@ __host__ __device__ __forceinline__ uint32_t expand_bits(uint32_t v) {
 	return v;
 }
 __host__ __device__ __forceinline__ uint32_t morton3D(uint32_t x, uint32_t y, uint32_t z) { return expand_bits(x) | (expand_bits(y) << 1) | (expand_bits(z) << 2); }
-__device__ __forceinline__ uint32_t cascaded_grid_idx_at(V3 pos, uint32_t mip) {  // :117-136
-	float mip_scale = __uint_as_float((127u - mip) << 23);  // scalbnf(1, -mip), exact
-	float px = fma_(sub(pos.x, 0.5f), mip_scale, 0.5f);
-	float py = fma_(sub(pos.y, 0.5f), mip_scale, 0.5f);
-	float pz = fma_(sub(pos.z, 0.5f), mip_scale, 0.5f);
-	int ix = (int)mul(px, 128.0f), iy = (int)mul(py, 128.0f), iz = (int)mul(pz, 128.0f);
-	ix = min(max(ix, 0), 127); iy = min(max(iy, 0), 127); iz = min(max(iz, 0), 127);
-	return morton3D((uint32_t)ix, (uint32_t)iy, (uint32_t)iz);
+// expand_bits for v < 128: the first stage, (v * 0x00010001) & 0xFF0000FF, is the identity on such v
+__device__ __forceinline__ uint32_t expand_bits7(uint32_t v) {
+	v = (v * 0x00000101u) & 0x0F00F00Fu;
+	v = (v * 0x00000011u) & 0xC30C30C3u;
+	v = (v * 0x00000005u) & 0x49249249u;
+	return v;
+}
+// expand_bits7(i) at index i < 128, for the march kernels' shared-memory copy: three loads replace the three multiply-mask chains
+__device__ __forceinline__ void fill_spread7(uint32_t* spread7) {
+	for (uint32_t i = threadIdx.x; i < 128; i += blockDim.x) spread7[i] = expand_bits7(i);
+}
+// the cell coordinates of cascaded_grid_idx_at, each clamped to 0..127
+__device__ __forceinline__ void cascaded_grid_coords(V3 pos, uint32_t mip, uint32_t& ix, uint32_t& iy, uint32_t& iz) {  // :117-136
+	// fma(a, 2^-mip, 0.5) * 128 == fma(a, 2^(7 - mip), 64) bit for bit: scaling by a power of two commutes with rounding, and
+	// neither side can overflow or underflow (|a| is bounded by the AABB; a nonzero sum is a multiple of ulp(a) * 2^-mip >= 2^-29)
+	float cell_scale = __uint_as_float((134u - mip) << 23);  // 2^(7 - mip), exact
+	float px = fma_(sub(pos.x, 0.5f), cell_scale, 64.0f);
+	float py = fma_(sub(pos.y, 0.5f), cell_scale, 64.0f);
+	float pz = fma_(sub(pos.z, 0.5f), cell_scale, 64.0f);
+	ix = (uint32_t)min(max((int)px, 0), 127); iy = (uint32_t)min(max((int)py, 0), 127); iz = (uint32_t)min(max((int)pz, 0), 127);
+}
+__device__ __forceinline__ uint32_t cascaded_grid_idx_at(V3 pos, uint32_t mip) {
+	uint32_t ix, iy, iz;
+	cascaded_grid_coords(pos, mip, ix, iy, iz);
+	return expand_bits7(ix) | (expand_bits7(iy) << 1) | (expand_bits7(iz) << 2);
+}
+// the same index with the 7-bit spread looked up in a fill_spread7 table
+__device__ __forceinline__ uint32_t cascaded_grid_idx_at(V3 pos, uint32_t mip, const uint32_t* spread7) {
+	uint32_t ix, iy, iz;
+	cascaded_grid_coords(pos, mip, ix, iy, iz);
+	return spread7[ix] | (spread7[iy] << 1) | (spread7[iz] << 2);
 }
 __device__ __forceinline__ bool bitfield_at(uint32_t idx, uint32_t mip, const uint8_t* __restrict__ bf) {
 	return (__ldg(bf + (idx >> 3) + mip * (GRIDVOL / 8)) & (1u << (idx & 7u))) != 0;
 }
-// exponent of frexpf(v) for v >= 0 (frexpf(0) -> 0)
-__device__ __forceinline__ int frexp_exp(float v) {
-	uint32_t b = __float_as_uint(v) & 0x7fffffffu;
-	if (b == 0) return 0;
-	int e = (int)(b >> 23);
-	if (e == 0) return (31 - __clz((int)b)) - 149 + 1;  // subnormal
-	return e - 126;
-}
 __device__ __forceinline__ int mip_from_pos(V3 pos) {  // :163-168
 	float maxval = fmaxf(fmaxf(fabsf(sub(pos.x, 0.5f)), fabsf(sub(pos.y, 0.5f))), fabsf(sub(pos.z, 0.5f)));
-	return min(CASCADES - 1, max(0, frexp_exp(maxval) + 1));
+	// clamp(frexp exponent + 1, 0, 4) from the exponent field e of maxval >= 0: a normal maxval gives e - 126 + 1; a subnormal has e = 0 and
+	// a frexp exponent <= -126, both clamp to 0; maxval == 0 (the exact AABB centre) is frexpf(0) + 1 = 1
+	const uint32_t b = __float_as_uint(maxval);
+	return b == 0 ? 1 : min(CASCADES - 1, max(0, (int)(b >> 23) - 125));
 }
 __device__ __forceinline__ int mip_from_dt(float dt, V3 pos) {  // :170-177
 	int mip = mip_from_pos(pos);
 	dt = mul(dt, 256.0f);
-	if (dt < 1.0f) return mip;
-	return min(CASCADES - 1, max(frexp_exp(dt), mip));
+	// dt >= 1 is normal, so its frexp exponent is (bits >> 23) - 126; below 1 the position's mip stands
+	const int e = dt < 1.0f ? 0 : (int)(__float_as_uint(dt) >> 23) - 126;
+	return min(CASCADES - 1, max(e, mip));
 }
 __device__ __forceinline__ float logistic_(float x) { return 1.0f / (1.0f + expf(-x)); }
 __device__ __forceinline__ float network_to_rgb(float v, int act) {  // :38-47
@@ -504,34 +535,35 @@ __device__ __noinline__ float4 glow_apply(int glow_mode, float glow_y_cutoff, V3
 }
 
 // Next occupied sample at or after t. false: the ray left the render AABB.
-__device__ __forceinline__ bool next_occupied(const DevFrame& f, const uint8_t* __restrict__ bitfield, V3 o, V3 d, V3 idir,
+// spread7: the block's fill_spread7 table in shared memory
+__device__ __forceinline__ bool next_occupied(const DevFrame& f, const uint8_t* __restrict__ bitfield, const uint32_t* spread7, V3 o, V3 d, V3 idir,
                                               float& t, float& dt, V3& pos, uint32_t& mip_out, uint32_t& cell_out) {
 	while (true) {
 		pos = madd3(d, t, o);
 		if (!box_contains(f.rmin, f.rmax, pos)) return false;
 		dt = calc_dt(t, f.cone);
 		uint32_t mip = (uint32_t)max(f.min_mip, mip_from_dt(dt, pos));
-		uint32_t cell = cascaded_grid_idx_at(pos, mip);
+		uint32_t cell = cascaded_grid_idx_at(pos, mip, spread7);
 		if (!bitfield || bitfield_at(cell, mip, bitfield)) { mip_out = mip; cell_out = cell; return true; }
-		t = advance_to_next_voxel(t, f.cone, pos, d, idir, GRIDSIZE >> mip);
+		t = advance_to_next_voxel(t, dt, f.cone, pos, d, idir, mip);
 	}
 }
 
 // The same walk, resumable: at most `budget` empty voxels are skipped per call. The state of the walk is `t`
 // alone (always a point of the ray's dt lattice), so splitting it over several calls yields bit-identical samples.
 enum MarchResult { MARCH_FOUND = 0, MARCH_EXIT = 1, MARCH_PENDING = 2 };
-__device__ __forceinline__ MarchResult next_occupied_budget(const DevFrame& f, const uint8_t* __restrict__ bitfield, V3 o, V3 d, V3 idir,
+__device__ __forceinline__ MarchResult next_occupied_budget(const DevFrame& f, const uint8_t* __restrict__ bitfield, const uint32_t* spread7, V3 o, V3 d, V3 idir,
                                                             float& t, float& dt, V3& pos, int& budget) {
 	while (true) {
 		pos = madd3(d, t, o);
 		if (!box_contains(f.rmin, f.rmax, pos)) return MARCH_EXIT;
 		dt = calc_dt(t, f.cone);
 		uint32_t mip = (uint32_t)max(f.min_mip, mip_from_dt(dt, pos));
-		uint32_t cell = cascaded_grid_idx_at(pos, mip);
+		uint32_t cell = cascaded_grid_idx_at(pos, mip, spread7);
 		if (!bitfield || bitfield_at(cell, mip, bitfield)) return MARCH_FOUND;
 		if (budget <= 0) return MARCH_PENDING;
 		--budget;
-		t = advance_to_next_voxel(t, f.cone, pos, d, idir, GRIDSIZE >> mip);
+		t = advance_to_next_voxel(t, dt, f.cone, pos, d, idir, mip);
 	}
 }
 

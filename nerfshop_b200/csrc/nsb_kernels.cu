@@ -55,6 +55,9 @@ template <bool GENERAL>
 __global__ void __launch_bounds__(256) k_prepare_rays(const DevFrame f, const uint8_t* __restrict__ bitfield, float4* __restrict__ fb, float* __restrict__ depth_out,
                                                       RayRec* __restrict__ list, float* __restrict__ ray_od, uint32_t* __restrict__ n_queued, uint32_t n_local_pixels,
                                                       unsigned long long* __restrict__ stats) {
+	__shared__ uint32_t spread7[128];
+	fill_spread7(spread7);
+	__syncthreads();
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	bool queued = false, is_ray = false, entered = false;
 	uint32_t pix = 0;
@@ -86,10 +89,10 @@ __global__ void __launch_bounds__(256) k_prepare_rays(const DevFrame f, const ui
 			}
 			if (inside) {
 				entered = true;
-				V3 idir = v3(div_(1.0f, r.d.x), div_(1.0f, r.d.y), div_(1.0f, r.d.z));
+				V3 idir = v3(__frcp_rn(r.d.x), __frcp_rn(r.d.y), __frcp_rn(r.d.z));
 				t = fma_(ld_random_val(f.spp, pix * 786433u), calc_dt(r.t, f.cone), r.t);  // advance_pos_nerf :585
 				float dt; V3 pos; uint32_t mip, cell;
-				queued = next_occupied(f, bitfield, r.o, r.d, idir, t, dt, pos, mip, cell);
+				queued = next_occupied(f, bitfield, spread7, r.o, r.d, idir, t, dt, pos, mip, cell);
 			}
 		}
 	}
@@ -173,6 +176,7 @@ template <int TILES>
 struct __align__(128) RenderSmemT {
 	uint8_t w[tc::W_BYTES];
 	TileBlock tile[TILES];
+	uint32_t spread7[128];  // fill_spread7: the march's Morton table
 	uint64_t w_bar;
 	uint32_t pad[2];
 };
@@ -201,6 +205,7 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 
 	// CTA setup: one bulk-TMA copy of the weight image
 	tc::load_weights(RS.w, &RS.w_bar, m.w_image);
+	fill_spread7(RS.spread7);
 	__syncthreads();
 	tc::mbar_wait(&RS.w_bar, 0);
 	tc::TileCtx C;
@@ -294,8 +299,9 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 			for (;;) {
 				if (!alive) break;
 				if (n_steps >= MARCH_ITER - 1) { alive = false; continue; }  // still marching after MARCH_ITER steps: dropped (:2812)
-				const V3 idir = v3(div_(1.0f, rd.x), div_(1.0f, rd.y), div_(1.0f, rd.z));
-				const MarchResult mr = next_occupied_budget(f, bitfield, ro, rd, idir, t, dt, pos, budget);
+				// __frcp_rn(x) == __fdiv_rn(1, x) bit for bit (the correctly rounded 1/x, ±0 -> ±inf), two instructions shorter
+				const V3 idir = v3(__frcp_rn(rd.x), __frcp_rn(rd.y), __frcp_rn(rd.z));
+				const MarchResult mr = next_occupied_budget(f, bitfield, RS.spread7, ro, rd, idir, t, dt, pos, budget);
 				if (mr == MARCH_FOUND) { has_sample = true; break; }
 				if (mr == MARCH_EXIT) {
 					finish(true, TB.ray[R_CR][tid], TB.ray[R_CG][tid], TB.ray[R_CB][tid], TB.ray[R_CA][tid], TB.ray[R_DEPTH][tid]);
@@ -319,7 +325,7 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 		bool need_old = false;
 		V3 pw_old = pw;
 		if (has_sample) {
-			pw = warp_position(pos, f.tmin, f.tmax);
+			pw = (!OPS && f.tinv_exact) ? warp_position_pow2(pos, f.tmin, f.tinv) : warp_position(pos, f.tmin, f.tmax);  // uniform branch; with operators it raised the spills
 			dtw = warp_dt(dt);
 			++n_steps;
 			++c_samples;
@@ -645,6 +651,9 @@ __global__ void k_poisson_residual_density(const DevOp* __restrict__ ops, int n_
 template <bool GENERAL>
 __global__ void k_march_trace(const DevFrame f, const uint8_t* __restrict__ bitfield, const uint32_t* __restrict__ pixels, uint32_t n_pixels,
                               uint32_t max_samples, float* __restrict__ rec, uint32_t* __restrict__ idx, uint32_t* __restrict__ count) {
+	__shared__ uint32_t spread7[128];
+	fill_spread7(spread7);
+	__syncthreads();
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n_pixels) return;
 	uint32_t pix = pixels[i];
@@ -652,11 +661,11 @@ __global__ void k_march_trace(const DevFrame f, const uint8_t* __restrict__ bitf
 	Ray r;
 	uint32_t c = 0;
 	if (GENERAL ? make_ray_general(f, px, py, r) : make_ray(f, px, py, r)) {
-		V3 idir = v3(div_(1.0f, r.d.x), div_(1.0f, r.d.y), div_(1.0f, r.d.z));
+		V3 idir = v3(__frcp_rn(r.d.x), __frcp_rn(r.d.y), __frcp_rn(r.d.z));
 		float t = fma_(ld_random_val(f.spp, pix * 786433u), calc_dt(r.t, f.cone), r.t);
 		while (c < MARCH_ITER) {
 			float dt; V3 pos; uint32_t mip, cell;
-			if (!next_occupied(f, bitfield, r.o, r.d, idir, t, dt, pos, mip, cell)) break;
+			if (!next_occupied(f, bitfield, spread7, r.o, r.d, idir, t, dt, pos, mip, cell)) break;
 			if (c < max_samples) {
 				float* rr = rec + ((size_t)i * max_samples + c) * 5;
 				rr[0] = t; rr[1] = dt; rr[2] = pos.x; rr[3] = pos.y; rr[4] = pos.z;
@@ -1675,6 +1684,18 @@ static NsbStatus to_dev_frame(const NsbFrame* f, DevFrame* d) {
 	memcpy(d->rs, f->rolling_shutter, sizeof(d->rs));
 	cp3(d->rmin, f->render_aabb_min); cp3(d->rmax, f->render_aabb_max);
 	cp3(d->tmin, f->train_aabb_min); cp3(d->tmax, f->train_aabb_max);
+	d->tinv_exact = 1;
+	for (int a = 0; a < 3; ++a) {  // the extent as the device computes it (one fp32 subtraction); 2^k with a normal 2^-k: store 2^-k
+		const float e = d->tmax[a] - d->tmin[a];
+		uint32_t b;
+		memcpy(&b, &e, sizeof(b));
+		const uint32_t ex = b >> 23;  // sign and exponent field: e > 0 has no sign bit
+		const bool pow2 = (b & 0x7fffffu) == 0 && ex >= 1 && ex <= 253;
+		const uint32_t ib = (254u - ex) << 23;
+		if (pow2) memcpy(&d->tinv[a], &ib, sizeof(ib));
+		else d->tinv[a] = 0.0f;
+		d->tinv_exact &= pow2 ? 1 : 0;
+	}
 	d->cone = f->cone_angle_constant;
 	d->min_T = f->min_transmittance;
 	d->depth_scale = f->depth_scale;
