@@ -17,7 +17,9 @@
  *
  * Conventions
  *  - plain pointers and sizes only; no exceptions cross the ABI; every call
- *    returns an NsbStatus and nsb_last_error() gives the message.
+ *    returns an NsbStatus and nsb_last_error() gives the message. After a
+ *    call fails with NSB_ERR_CUDA because an allocation failed, the context
+ *    can still be used, and any model or operator it reports is intact.
  *  - "host" pointers are read during the call and never retained.
  *  - "dev" pointers are CUDA device pointers owned by the caller.
  *  - matrices are column-major like Eigen (camera 3x4: 12 floats, col 0..3).

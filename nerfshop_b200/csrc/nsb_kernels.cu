@@ -14,7 +14,9 @@
 #include <cstdlib>
 #include <cstring>
 #include <ctime>
+#include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/nerfshop_b200.h"
@@ -936,6 +938,31 @@ static NsbStatus fail(NsbStatus s, const char* fmt, ...) {
 		if (e__ != cudaSuccess) return fail(NSB_ERR_CUDA, "%s: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
 	} while (0)
 
+// Owner of one device array of T. reserve() only grows and does not keep the contents. A failed reserve leaves the buffer empty
+// (null, capacity 0), so a buffer never reports room it does not have.
+template <typename T>
+class DevBuf {
+	T* p_ = nullptr;
+	size_t n_ = 0;  // capacity in elements
+
+public:
+	DevBuf() = default;
+	DevBuf(DevBuf&& o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+	DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p_, o.p_); std::swap(n_, o.n_); return *this; }  // the old array goes with o
+	~DevBuf() { cudaFree(p_); }
+	cudaError_t reserve(size_t n) {
+		if (n <= n_) return cudaSuccess;
+		cudaFree(p_);
+		n_ = 0;
+		const cudaError_t e = cudaMalloc(&p_, n * sizeof(T));
+		if (e == cudaSuccess) n_ = n;
+		else p_ = nullptr;
+		return e;
+	}
+	T* get() const { return p_; }
+	size_t capacity() const { return n_; }
+};
+
 struct NsbContext {
 	int device = 0;
 	int sm_count = 0;
@@ -944,51 +971,54 @@ struct NsbContext {
 	bool has_model = false, has_occ = false;
 	NsbModelDesc desc{};
 	DevModel model{};
-	__half2* d_grid = nullptr;
-	uint8_t* d_wimage = nullptr;
-	__half* d_wrow = nullptr;
-	uint8_t* d_bitfield = nullptr;
-	float* d_density_grid = nullptr;   // running density grid, 5 x 128^3 (Testbed::Nerf::density_grid, testbed.h:622)
-	float* d_density_tmp = nullptr;    // density_grid_tmp scratch of an update
-	double* d_mean_partial = nullptr;
-	float* d_thresh = nullptr;         // [0] bitfield threshold, [1] mean of cascade 0
-	DevOp* d_ops = nullptr;
+	DevBuf<__half2> d_grid;
+	DevBuf<uint8_t> d_wimage;
+	DevBuf<__half> d_wrow;
+	DevBuf<uint8_t> d_bitfield;
+	DevBuf<float> d_density_grid;      // running density grid, 5 x 128^3 (Testbed::Nerf::density_grid, testbed.h:622)
+	DevBuf<float> d_density_tmp;       // density_grid_tmp scratch of an update
+	DevBuf<double> d_mean_partial;
+	DevBuf<float> d_thresh;            // [0] bitfield threshold, [1] mean of cascade 0
+	DevBuf<DevOp> d_ops;
 	int n_ops = 0;
 	int any_poisson = 0;
-	std::vector<void*> op_allocs;
 	std::vector<DevOp> h_ops;          // host copy of d_ops (pointers are device pointers)
-	struct CageRebuild {               // device scratch of nsb_cage_deform, one per operator slot
-		float* d_mvc = nullptr; uint32_t n_cv = 0, n_vertices = 0;
-		float* d_cage = nullptr;
-		uint32_t* d_counts = nullptr; uint32_t* d_block_sums = nullptr; uint32_t* d_total = nullptr;
-		nsb::rebuild::Mark* d_marks = nullptr; uint32_t marks_cap = 0; unsigned int* d_n_marks = nullptr;
-		uint32_t* d_idx = nullptr; uint64_t idx_cap = 0;   // owned replacement of the uploaded tet_lut_idx once it had to grow
-		float* d_boxes = nullptr;      // [12] bbox min/max, warped min/max; [12..17] scene aabb
-		float* d_gamma = nullptr; float* d_mem_small = nullptr; uint32_t mem_n_cv = 0;  // nsb_cage_set_membrane scratch
-		uint64_t n_idx = 0;
+	struct CageArrays {                // device arrays of one operator slot (empty for an affine operator)
+		// what the slot's DevOp points at, as uploaded by nsb_set_edit_ops; nsb_cage_deform rewrites verts/rots/lut_* in place
+		DevBuf<uint32_t> lut_off, lut_idx, tets;
+		DevBuf<float> verts, orig_verts, rots, shs, od, rd;
+		DevBuf<uint8_t> obits;
+		uint32_t n_vertices = 0;
+		uint64_t n_idx = 0;            // entries of lut_idx in use
+		// nsb_cage_attach_mvc / nsb_cage_deform
+		DevBuf<float> d_mvc; uint32_t n_cv = 0;
+		DevBuf<float> d_cage;
+		DevBuf<uint32_t> d_counts, d_block_sums, d_total;
+		DevBuf<nsb::rebuild::Mark> d_marks; DevBuf<unsigned int> d_n_marks;
+		DevBuf<float> d_boxes;         // [12] bbox min/max, warped min/max; [12..17] scene aabb
+		DevBuf<float> d_gamma, d_mem_small;  // nsb_cage_set_membrane scratch
 	};
-	std::vector<CageRebuild> rb;
-	uint32_t* d_counters = nullptr;  // [0] rays queued by k_prepare_rays, [1] fetch cursor of k_render_fused
-	unsigned long long* d_stats = nullptr;
-	RayRec* d_list = nullptr;
-	size_t list_capacity = 0;
-	float* d_ray_od = nullptr;     // origin + direction per queue slot, general-camera frames only (allocated on the first such frame)
-	size_t ray_od_capacity = 0;
+	std::vector<CageArrays> rb;
+	DevBuf<uint32_t> d_counters;       // [0] rays queued by k_prepare_rays, [1] fetch cursor of k_render_fused
+	DevBuf<unsigned long long> d_stats;
+	DevBuf<RayRec> d_list;
+	DevBuf<float> d_ray_od;            // origin + direction per queue slot, general-camera frames only (allocated on the first such frame)
 	int acc16 = 1;                 // MLP accumulator policy: 1 fp16 wgmma accumulators (default: the reference's wmma __half fragments), 0 fp32 (nsb_set_mlp_accumulator)
 	cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr;  // start, end, between k_prepare_rays and k_render_fused
 	bool timed = false;
 	uint32_t launches = 0;
-	float* d_fb = nullptr;
-	float* d_depth = nullptr;
-	size_t fb_pixels = 0;
+	DevBuf<float> d_fb, d_depth;       // nsb_render_host
 	cudaStream_t stream = nullptr;
 	// nsb_render_host_async: two framebuffers in flight, the D2H copy of one overlaps the render of the other
-	float* d_fb2[2] = {nullptr, nullptr};
-	float* d_depth2[2] = {nullptr, nullptr};
-	size_t fb2_pixels = 0;
+	DevBuf<float> d_fb2[2], d_depth2[2];
 	cudaStream_t copy_stream = nullptr;
 	cudaEvent_t render_done[2] = {nullptr, nullptr}, copy_done[2] = {nullptr, nullptr};
 	uint64_t host_seq = 0;  // tickets issued
+
+	~NsbContext() {  // the device arrays free themselves
+		for (cudaEvent_t e : {ev0, ev1, evm, render_done[0], render_done[1], copy_done[0], copy_done[1]}) if (e) cudaEventDestroy(e);
+		for (cudaStream_t s : {stream, copy_stream}) if (s) cudaStreamDestroy(s);
+	}
 };
 
 static uint32_t next_multiple_u32(uint32_t v, uint32_t m) { return ((v + m - 1) / m) * m; }
@@ -1045,12 +1075,12 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 	cudaDeviceProp prop;
 	CU(cudaGetDeviceProperties(&prop, device));
 	if (prop.major != 9 || prop.minor != 0) return fail(NSB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
-	NsbContext* c = new NsbContext();
+	std::unique_ptr<NsbContext> c(new NsbContext());  // released to the caller only once complete
 	c->device = device;
 	c->sm_count = prop.multiProcessorCount;
-	CU(cudaMalloc(&c->d_counters, 2 * sizeof(uint32_t)));
-	CU(cudaMalloc(&c->d_stats, ST_N * sizeof(unsigned long long)));
-	CU(cudaMemset(c->d_stats, 0, ST_N * sizeof(unsigned long long)));
+	CU(c->d_counters.reserve(2));
+	CU(c->d_stats.reserve(ST_N));
+	CU(cudaMemset(c->d_stats.get(), 0, ST_N * sizeof(unsigned long long)));
 	CU(cudaEventCreate(&c->ev0));
 	CU(cudaEventCreate(&c->ev1));
 	CU(cudaEventCreate(&c->evm));
@@ -1102,43 +1132,14 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 	if (getenv("NSB_VERBOSE"))
 		fprintf(stderr, "[nsb] device %d: %d SMs; k_render_fused %d tiles/CTA (%d with operators), %d regs, %zu B smem; inference %d CTAs/SM, grid update %d CTAs/SM\n", device, c->sm_count,
 		        render_tiles(false), render_tiles(true), fa.numRegs, sizeof(RenderSmemT<render_tiles(false)>), c->inference_ctas_per_sm, c->grid_update_ctas_per_sm);
-	*out = c;
+	*out = c.release();
 	return NSB_OK;
-}
-
-static void free_ops(NsbContext* c) {
-	for (void* p : c->op_allocs) cudaFree(p);
-	c->op_allocs.clear();
-	for (auto& r : c->rb) {
-		cudaFree(r.d_mvc); cudaFree(r.d_cage); cudaFree(r.d_counts); cudaFree(r.d_block_sums); cudaFree(r.d_total); cudaFree(r.d_marks);
-		cudaFree(r.d_n_marks); cudaFree(r.d_idx); cudaFree(r.d_boxes); cudaFree(r.d_gamma); cudaFree(r.d_mem_small);
-	}
-	c->rb.clear();
-	c->h_ops.clear();
-	if (c->d_ops) cudaFree(c->d_ops);
-	c->d_ops = nullptr;
-	c->n_ops = 0;
-	c->any_poisson = 0;
 }
 
 extern "C" NsbStatus nsb_destroy(NsbContext* c) {
 	if (!c) return NSB_OK;
 	cudaSetDevice(c->device);
 	cudaDeviceSynchronize();
-	free_ops(c);
-	cudaFree(c->d_grid); cudaFree(c->d_wimage); cudaFree(c->d_wrow); cudaFree(c->d_bitfield);
-	cudaFree(c->d_density_grid); cudaFree(c->d_density_tmp); cudaFree(c->d_mean_partial); cudaFree(c->d_thresh);
-	cudaFree(c->d_counters); cudaFree(c->d_stats); cudaFree(c->d_fb); cudaFree(c->d_depth); cudaFree(c->d_list); cudaFree(c->d_ray_od);
-	if (c->ev0) cudaEventDestroy(c->ev0);
-	if (c->ev1) cudaEventDestroy(c->ev1);
-	if (c->evm) cudaEventDestroy(c->evm);
-	if (c->stream) cudaStreamDestroy(c->stream);
-	if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-	for (int i = 0; i < 2; ++i) {
-		if (c->render_done[i]) cudaEventDestroy(c->render_done[i]);
-		if (c->copy_done[i]) cudaEventDestroy(c->copy_done[i]);
-		cudaFree(c->d_fb2[i]); cudaFree(c->d_depth2[i]);
-	}
 	delete c;
 	return NSB_OK;
 }
@@ -1161,8 +1162,10 @@ static NsbStatus upload_model_impl(NsbContext* c, const NsbModelDesc* desc, cons
 	if (!build_levels(desc, m.levels, &n_grid)) return fail(NSB_ERR_INVALID, "unsupported model description (only the configs/nerf/base.json topology is implemented)");
 	if (n_params != kMlpParams + 2 * n_grid) return fail(NSB_ERR_INVALID, "n_params %llu != expected %llu", (unsigned long long)n_params, (unsigned long long)(kMlpParams + 2 * n_grid));
 	CU(cudaDeviceSynchronize());
-	cudaFree(c->d_grid); cudaFree(c->d_wimage); cudaFree(c->d_wrow);
-	c->d_grid = nullptr; c->d_wimage = nullptr; c->d_wrow = nullptr;
+	// has_model implies that model points into live buffers: it is cleared before the old model's buffers are released, and set again
+	// only once the new model is complete
+	c->has_model = false;
+	c->d_grid = {}; c->d_wimage = {}; c->d_wrow = {};
 	// block order: density MLP, rgb MLP, hash grid (nerf_network_full.h:316-349)
 	std::vector<uint8_t> image(tc::W_BYTES);
 	std::vector<uint16_t> mlp_host;
@@ -1176,16 +1179,16 @@ static NsbStatus upload_model_impl(NsbContext* c, const NsbModelDesc* desc, cons
 	to_operand_layout(w, 64, 32, image.data() + tc::W3_OFF); w += 64 * 32;
 	to_operand_layout(w, 64, 64, image.data() + tc::W4_OFF); w += 64 * 64;
 	to_operand_layout(w, 16, 64, image.data() + tc::W5_OFF); w += 16 * 64;
-	CU(cudaMalloc(&c->d_wimage, tc::W_BYTES));
-	CU(cudaMemcpy(c->d_wimage, image.data(), tc::W_BYTES, cudaMemcpyHostToDevice));
-	CU(cudaMalloc(&c->d_wrow, kMlpParams * 2));
-	CU(cudaMemcpy(c->d_wrow, params, kMlpParams * 2, params_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
-	CU(cudaMalloc(&c->d_grid, n_grid * 4));
-	CU(cudaMemcpy(c->d_grid, params + kMlpParams, n_grid * 4, params_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
-	m.grid = c->d_grid;
-	for (uint32_t l = 0; l < desc->n_levels; ++l) m.levels[l].base = c->d_grid + (uintptr_t)m.levels[l].base / sizeof(__half2);
-	m.w_image = c->d_wimage;
-	m.w_rowmajor = c->d_wrow;
+	CU(c->d_wimage.reserve(tc::W_BYTES));
+	CU(cudaMemcpy(c->d_wimage.get(), image.data(), tc::W_BYTES, cudaMemcpyHostToDevice));
+	CU(c->d_wrow.reserve(kMlpParams));
+	CU(cudaMemcpy(c->d_wrow.get(), params, kMlpParams * 2, params_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+	CU(c->d_grid.reserve(n_grid));
+	CU(cudaMemcpy(c->d_grid.get(), params + kMlpParams, n_grid * 4, params_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+	m.grid = c->d_grid.get();
+	for (uint32_t l = 0; l < desc->n_levels; ++l) m.levels[l].base = c->d_grid.get() + (uintptr_t)m.levels[l].base / sizeof(__half2);
+	m.w_image = c->d_wimage.get();
+	m.w_rowmajor = c->d_wrow.get();
 	m.n_levels = desc->n_levels;
 	for (int g = 0; g < MAX_LEVELS / 2; ++g) {
 		uint32_t a = m.levels[2 * g].hashed, b = m.levels[2 * g + 1].hashed;
@@ -1208,9 +1211,9 @@ static NsbStatus upload_occupancy_impl(NsbContext* c, const uint8_t* bitfield, u
 	if (!c || !bitfield) return fail(NSB_ERR_INVALID, "null argument");
 	if (n_bytes != NSB_BITFIELD_BYTES) return fail(NSB_ERR_INVALID, "bitfield must be %u bytes (5 x 128^3 / 8)", NSB_BITFIELD_BYTES);
 	CU(cudaSetDevice(c->device));
-	if (!c->d_bitfield) CU(cudaMalloc(&c->d_bitfield, NSB_BITFIELD_BYTES));
+	CU(c->d_bitfield.reserve(NSB_BITFIELD_BYTES));
 	CU(cudaDeviceSynchronize());
-	CU(cudaMemcpy(c->d_bitfield, bitfield, NSB_BITFIELD_BYTES, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+	CU(cudaMemcpy(c->d_bitfield.get(), bitfield, NSB_BITFIELD_BYTES, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
 	c->has_occ = true;
 	return NSB_OK;
 }
@@ -1219,24 +1222,27 @@ extern "C" NsbStatus nsb_upload_occupancy_dev(NsbContext* c, const uint8_t* bitf
 
 static NsbStatus ensure_grid_buffers(NsbContext* c) {
 	const uint32_t n_blocks = (GRIDVOL + 256 * 64 - 1) / (256 * 64);
-	if (!c->d_density_grid) {
-		CU(cudaMalloc(&c->d_density_grid, (size_t)NSB_GRID_CELLS * 4));
-		CU(cudaMemset(c->d_density_grid, 0, (size_t)NSB_GRID_CELLS * 4));
+	if (!c->d_density_grid.get()) {  // the grid is either zeroed or not allocated: it joins the context once zeroed
+		DevBuf<float> grid;
+		CU(grid.reserve(NSB_GRID_CELLS));
+		CU(cudaMemset(grid.get(), 0, (size_t)NSB_GRID_CELLS * 4));
+		c->d_density_grid = std::move(grid);
 	}
-	if (!c->d_mean_partial) CU(cudaMalloc(&c->d_mean_partial, n_blocks * sizeof(double)));
-	if (!c->d_thresh) CU(cudaMalloc(&c->d_thresh, 2 * sizeof(float)));
-	if (!c->d_bitfield) CU(cudaMalloc(&c->d_bitfield, NSB_BITFIELD_BYTES));
+	CU(c->d_mean_partial.reserve(n_blocks));
+	CU(c->d_thresh.reserve(2));
+	CU(c->d_bitfield.reserve(NSB_BITFIELD_BYTES));
 	return NSB_OK;
 }
 // Testbed::update_density_grid_mean_and_bitfield (testbed_nerf.cu:3642-3658), device-resident and stream-ordered
 static NsbStatus rebuild_bitfield(NsbContext* c, cudaStream_t st) {
 	const uint32_t n0 = GRIDVOL, n_blocks = (n0 + 256 * 64 - 1) / (256 * 64);
-	k_grid_mean_partial<<<n_blocks, 256, 0, st>>>(c->d_density_grid, n0, c->d_mean_partial);  // reduce_sum(fmaxf(val,0)/n) over cascade 0 (:3650)
-	k_grid_mean_final<<<1, 1, 0, st>>>(c->d_mean_partial, n_blocks, n0, c->d_thresh);
-	k_grid_to_bitfield_dev<<<(NSB_BITFIELD_BYTES + 255) / 256, 256, 0, st>>>(NSB_BITFIELD_BYTES, c->d_density_grid, c->d_bitfield, c->d_thresh);
+	k_grid_mean_partial<<<n_blocks, 256, 0, st>>>(c->d_density_grid.get(), n0, c->d_mean_partial.get());  // reduce_sum(fmaxf(val,0)/n) over cascade 0 (:3650)
+	k_grid_mean_final<<<1, 1, 0, st>>>(c->d_mean_partial.get(), n_blocks, n0, c->d_thresh.get());
+	k_grid_to_bitfield_dev<<<(NSB_BITFIELD_BYTES + 255) / 256, 256, 0, st>>>(NSB_BITFIELD_BYTES, c->d_density_grid.get(), c->d_bitfield.get(), c->d_thresh.get());
 	for (uint32_t level = 1; level < NSB_NERF_CASCADES; ++level) {
 		const uint32_t n = GRIDVOL / 64;
-		k_bitfield_max_pool<<<(n + 255) / 256, 256, 0, st>>>(n, c->d_bitfield + (size_t)(level - 1) * (GRIDVOL / 8), c->d_bitfield + (size_t)level * (GRIDVOL / 8));
+		uint8_t* bits = c->d_bitfield.get();
+		k_bitfield_max_pool<<<(n + 255) / 256, 256, 0, st>>>(n, bits + (size_t)(level - 1) * (GRIDVOL / 8), bits + (size_t)level * (GRIDVOL / 8));
 	}
 	CU(cudaGetLastError());
 	c->has_occ = true;
@@ -1250,11 +1256,11 @@ extern "C" NsbStatus nsb_upload_density_grid(NsbContext* c, const float* grid, u
 	CU(cudaDeviceSynchronize());
 	NsbStatus st = ensure_grid_buffers(c);
 	if (st != NSB_OK) return st;
-	CU(cudaMemcpy(c->d_density_grid, grid, n_floats * 4, cudaMemcpyHostToDevice));
+	CU(cudaMemcpy(c->d_density_grid.get(), grid, n_floats * 4, cudaMemcpyHostToDevice));
 	st = rebuild_bitfield(c, nullptr);
 	if (st != NSB_OK) return st;
 	CU(cudaDeviceSynchronize());
-	if (bitfield_out) CU(cudaMemcpy(bitfield_out, c->d_bitfield, NSB_BITFIELD_BYTES, cudaMemcpyDeviceToHost));
+	if (bitfield_out) CU(cudaMemcpy(bitfield_out, c->d_bitfield.get(), NSB_BITFIELD_BYTES, cudaMemcpyDeviceToHost));
 	return NSB_OK;
 }
 
@@ -1268,9 +1274,9 @@ extern "C" NsbStatus nsb_update_density_grid(NsbContext* c, const NsbGridUpdate*
 	cudaStream_t st = (cudaStream_t)stream_;
 	NsbStatus rc = ensure_grid_buffers(c);
 	if (rc != NSB_OK) return rc;
-	if (!c->d_density_tmp) CU(cudaMalloc(&c->d_density_tmp, (size_t)NSB_GRID_CELLS * 4));
-	if (u->reset_grid) CU(cudaMemsetAsync(c->d_density_grid, 0, (size_t)NSB_GRID_CELLS * 4, st));        // :3558-3560
-	CU(cudaMemsetAsync(c->d_density_tmp, 0, (size_t)NSB_GRID_CELLS * 4, st));                            // :3563
+	CU(c->d_density_tmp.reserve(NSB_GRID_CELLS));
+	if (u->reset_grid) CU(cudaMemsetAsync(c->d_density_grid.get(), 0, (size_t)NSB_GRID_CELLS * 4, st));  // :3558-3560
+	CU(cudaMemsetAsync(c->d_density_tmp.get(), 0, (size_t)NSB_GRID_CELLS * 4, st));                      // :3563
 	const uint32_t n_total = (uint32_t)n_total64;
 	if (n_total > 0) {
 		GridUpdateArgs a{};
@@ -1281,9 +1287,9 @@ extern "C" NsbStatus nsb_update_density_grid(NsbContext* c, const NsbGridUpdate*
 		uint32_t grid = (n_total + 127u) / 128u;
 		uint32_t cap = (uint32_t)(c->sm_count * c->grid_update_ctas_per_sm);
 		if (grid > cap) grid = cap;
-		(c->acc16 ? k_density_grid_update<true> : k_density_grid_update<false>)<<<grid, 128, sizeof(tc::TileSmem), st>>>(c->model, c->d_ops, c->n_ops, a, c->d_density_grid, c->d_density_tmp);
+		(c->acc16 ? k_density_grid_update<true> : k_density_grid_update<false>)<<<grid, 128, sizeof(tc::TileSmem), st>>>(c->model, c->d_ops.get(), c->n_ops, a, c->d_density_grid.get(), c->d_density_tmp.get());
 	}
-	k_ema_grid<<<(NSB_GRID_CELLS + 255) / 256, 256, 0, st>>>((uint32_t)NSB_GRID_CELLS, u->decay, c->d_density_grid, c->d_density_tmp);  // :3634
+	k_ema_grid<<<(NSB_GRID_CELLS + 255) / 256, 256, 0, st>>>((uint32_t)NSB_GRID_CELLS, u->decay, c->d_density_grid.get(), c->d_density_tmp.get());  // :3634
 	CU(cudaGetLastError());
 	return rebuild_bitfield(c, st);                                                                      // :3639
 }
@@ -1293,25 +1299,23 @@ extern "C" NsbStatus nsb_download_density_grid(NsbContext* c, float* grid_out, u
 	CU(cudaSetDevice(c->device));
 	CU(cudaDeviceSynchronize());
 	if (grid_out) {
-		if (!c->d_density_grid) return fail(NSB_ERR_STATE, "no density grid: call nsb_upload_density_grid or nsb_update_density_grid first");
-		CU(cudaMemcpy(grid_out, c->d_density_grid, (size_t)NSB_GRID_CELLS * 4, cudaMemcpyDeviceToHost));
+		if (!c->d_density_grid.get()) return fail(NSB_ERR_STATE, "no density grid: call nsb_upload_density_grid or nsb_update_density_grid first");
+		CU(cudaMemcpy(grid_out, c->d_density_grid.get(), (size_t)NSB_GRID_CELLS * 4, cudaMemcpyDeviceToHost));
 	}
 	if (bitfield_out) {
-		if (!c->d_bitfield || !c->has_occ) return fail(NSB_ERR_STATE, "no occupancy bitfield");
-		CU(cudaMemcpy(bitfield_out, c->d_bitfield, NSB_BITFIELD_BYTES, cudaMemcpyDeviceToHost));
+		if (!c->d_bitfield.get() || !c->has_occ) return fail(NSB_ERR_STATE, "no occupancy bitfield");
+		CU(cudaMemcpy(bitfield_out, c->d_bitfield.get(), NSB_BITFIELD_BYTES, cudaMemcpyDeviceToHost));
 	}
 	return NSB_OK;
 }
 
 template <typename T>
-static NsbStatus dev_copy(NsbContext* c, const T* host, size_t count, const T** out) {
+static NsbStatus dev_copy(DevBuf<T>& buf, const T* host, size_t count, const T** out) {
 	*out = nullptr;
 	if (!host || count == 0) return NSB_OK;
-	void* p = nullptr;
-	CU(cudaMalloc(&p, count * sizeof(T)));
-	c->op_allocs.push_back(p);
-	CU(cudaMemcpy(p, host, count * sizeof(T), cudaMemcpyHostToDevice));
-	*out = reinterpret_cast<const T*>(p);
+	CU(buf.reserve(count));
+	CU(cudaMemcpy(buf.get(), host, count * sizeof(T), cudaMemcpyHostToDevice));
+	*out = buf.get();
 	return NSB_OK;
 }
 static void cp3(float* d, const float* s) { d[0] = s[0]; d[1] = s[1]; d[2] = s[2]; }
@@ -1321,13 +1325,19 @@ extern "C" NsbStatus nsb_set_edit_ops(NsbContext* c, const NsbEditOp* ops, int32
 	if (!c || n < 0 || (n > 0 && !ops)) return fail(NSB_ERR_INVALID, "bad arguments");
 	CU(cudaSetDevice(c->device));
 	CU(cudaDeviceSynchronize());
-	free_ops(c);
+	// the old operators go first; the new ones are built in locals and join the context only once complete
+	c->n_ops = c->any_poisson = 0;
+	c->h_ops.clear();
+	c->rb.clear();
+	c->d_ops = {};
 	if (n == 0) return NSB_OK;
 	std::vector<DevOp> dev(n);
+	std::vector<NsbContext::CageArrays> rb(n);
 	int any_poisson = 0;
 	for (int i = 0; i < n; ++i) {
 		const NsbEditOp& s = ops[i];
 		DevOp& d = dev[i];
+		auto& r = rb[i];
 		memset(&d, 0, sizeof(d));
 		d.type = s.type;
 		if (s.type == NSB_OP_CAGE) {
@@ -1339,23 +1349,23 @@ extern "C" NsbStatus nsb_set_edit_ops(NsbContext* c, const NsbEditOp* ops, int32
 			cp3(d.wbmin, s.warped_bbox_min); cp3(d.wbmax, s.warped_bbox_max);
 			cp3(d.owbmin, s.original_warped_bbox_min); cp3(d.owbmax, s.original_warped_bbox_max);
 			d.n_tets = s.n_tets;
+			r.n_vertices = s.n_vertices;
+			r.n_idx = s.n_lut_idx;
 			if (s.n_tets) {
-				if (!s.tet_lut_offsets || !s.tets || !s.vertices || !s.original_vertices || !s.original_bitfield || (s.n_lut_idx && !s.tet_lut_idx)) {
-					free_ops(c);
+				if (!s.tet_lut_offsets || !s.tets || !s.vertices || !s.original_vertices || !s.original_bitfield || (s.n_lut_idx && !s.tet_lut_idx))
 					return fail(NSB_ERR_INVALID, "cage operator %d: missing arrays", i);
-				}
 				NsbStatus st;
-				if ((st = dev_copy(c, s.tet_lut_offsets, (size_t)NSB_GRID_CELLS + 1, &d.lut_off)) != NSB_OK) return st;
-				if ((st = dev_copy(c, s.tet_lut_idx, (size_t)s.n_lut_idx, &d.lut_idx)) != NSB_OK) return st;
-				if ((st = dev_copy(c, s.tets, (size_t)4 * s.n_tets, &d.tets)) != NSB_OK) return st;
-				if ((st = dev_copy(c, s.vertices, (size_t)3 * s.n_vertices, &d.verts)) != NSB_OK) return st;
-				if ((st = dev_copy(c, s.original_vertices, (size_t)3 * s.n_vertices, &d.orig_verts)) != NSB_OK) return st;
-				if ((st = dev_copy(c, s.local_rotations, (size_t)9 * s.n_tets, &d.rots)) != NSB_OK) return st;
-				if ((st = dev_copy(c, s.original_bitfield, (size_t)NSB_BITFIELD_BYTES, &d.obits)) != NSB_OK) return st;
+				if ((st = dev_copy(r.lut_off, s.tet_lut_offsets, (size_t)NSB_GRID_CELLS + 1, &d.lut_off)) != NSB_OK) return st;
+				if ((st = dev_copy(r.lut_idx, s.tet_lut_idx, (size_t)s.n_lut_idx, &d.lut_idx)) != NSB_OK) return st;
+				if ((st = dev_copy(r.tets, s.tets, (size_t)4 * s.n_tets, &d.tets)) != NSB_OK) return st;
+				if ((st = dev_copy(r.verts, s.vertices, (size_t)3 * s.n_vertices, &d.verts)) != NSB_OK) return st;
+				if ((st = dev_copy(r.orig_verts, s.original_vertices, (size_t)3 * s.n_vertices, &d.orig_verts)) != NSB_OK) return st;
+				if ((st = dev_copy(r.rots, s.local_rotations, (size_t)9 * s.n_tets, &d.rots)) != NSB_OK) return st;
+				if ((st = dev_copy(r.obits, s.original_bitfield, (size_t)NSB_BITFIELD_BYTES, &d.obits)) != NSB_OK) return st;
 				if (s.boundary_shs && s.boundary_outside_density && s.boundary_residual_density) {
-					if ((st = dev_copy(c, s.boundary_shs, (size_t)27 * s.n_vertices, &d.shs)) != NSB_OK) return st;
-					if ((st = dev_copy(c, s.boundary_outside_density, (size_t)s.n_vertices, &d.od)) != NSB_OK) return st;
-					if ((st = dev_copy(c, s.boundary_residual_density, (size_t)s.n_vertices, &d.rd)) != NSB_OK) return st;
+					if ((st = dev_copy(r.shs, s.boundary_shs, (size_t)27 * s.n_vertices, &d.shs)) != NSB_OK) return st;
+					if ((st = dev_copy(r.od, s.boundary_outside_density, (size_t)s.n_vertices, &d.od)) != NSB_OK) return st;
+					if ((st = dev_copy(r.rd, s.boundary_residual_density, (size_t)s.n_vertices, &d.rd)) != NSB_OK) return st;
 					d.has_poisson_data = 1;
 				}
 				if (d.apply_poisson && d.has_poisson_data) any_poisson = 1;
@@ -1369,17 +1379,17 @@ extern "C" NsbStatus nsb_set_edit_ops(NsbContext* c, const NsbEditOp* ops, int32
 			d.hide_original = s.hide_original;
 			d.correct_dir = s.correct_dir;
 		} else {
-			free_ops(c);
 			return fail(NSB_ERR_INVALID, "operator %d: unknown type %d", i, s.type);
 		}
 	}
-	CU(cudaMalloc(&c->d_ops, sizeof(DevOp) * n));
-	CU(cudaMemcpy(c->d_ops, dev.data(), sizeof(DevOp) * n, cudaMemcpyHostToDevice));
+	DevBuf<DevOp> d_ops;
+	CU(d_ops.reserve(n));
+	CU(cudaMemcpy(d_ops.get(), dev.data(), sizeof(DevOp) * n, cudaMemcpyHostToDevice));
+	c->d_ops = std::move(d_ops);
+	c->rb = std::move(rb);
+	c->h_ops = std::move(dev);
 	c->n_ops = n;
 	c->any_poisson = any_poisson;
-	c->h_ops = dev;
-	c->rb.assign((size_t)n, NsbContext::CageRebuild{});
-	for (int i = 0; i < n; ++i) { c->rb[i].n_vertices = ops[i].type == NSB_OP_CAGE ? ops[i].n_vertices : 0; c->rb[i].n_idx = c->rb[i].idx_cap = ops[i].type == NSB_OP_CAGE ? ops[i].n_lut_idx : 0; }
 	return NSB_OK;
 }
 
@@ -1396,12 +1406,14 @@ extern "C" NsbStatus nsb_cage_attach_mvc(NsbContext* c, int32_t op_index, const 
 	if (!weights || n_cage_vertices == 0 || n_cage_vertices > 4096) return fail(NSB_ERR_INVALID, "nsb_cage_attach_mvc: bad weights / cage size");
 	CU(cudaSetDevice(c->device));
 	auto& r = c->rb[op_index];
-	cudaFree(r.d_mvc); cudaFree(r.d_cage);
-	r.d_mvc = nullptr; r.d_cage = nullptr;
+	// the weights are either copied in or not allocated: the old ones go first, and the new ones join the operator once copied
+	r.d_mvc = {}; r.d_cage = {};
+	DevBuf<float> mvc;
+	CU(mvc.reserve((size_t)r.n_vertices * n_cage_vertices));
+	CU(r.d_cage.reserve((size_t)3 * n_cage_vertices));
+	CU(cudaMemcpy(mvc.get(), weights, (size_t)r.n_vertices * n_cage_vertices * sizeof(float), cudaMemcpyHostToDevice));
+	r.d_mvc = std::move(mvc);
 	r.n_cv = n_cage_vertices;
-	CU(cudaMalloc(&r.d_mvc, (size_t)r.n_vertices * n_cage_vertices * sizeof(float)));
-	CU(cudaMalloc(&r.d_cage, (size_t)3 * n_cage_vertices * sizeof(float)));
-	CU(cudaMemcpy(r.d_mvc, weights, (size_t)r.n_vertices * n_cage_vertices * sizeof(float), cudaMemcpyHostToDevice));
 	return NSB_OK;
 }
 extern "C" NsbStatus nsb_cage_deform(NsbContext* c, int32_t op_index, const float* cage_vertices, uint32_t n_cage_vertices, void* stream_) {
@@ -1409,81 +1421,82 @@ extern "C" NsbStatus nsb_cage_deform(NsbContext* c, int32_t op_index, const floa
 	NsbStatus st = cage_slot(c, op_index, "nsb_cage_deform");
 	if (st != NSB_OK) return st;
 	auto& r = c->rb[op_index];
-	if (!r.d_mvc) return fail(NSB_ERR_STATE, "nsb_cage_deform: nsb_cage_attach_mvc has not been called for operator %d", op_index);
+	if (!r.d_mvc.get()) return fail(NSB_ERR_STATE, "nsb_cage_deform: nsb_cage_attach_mvc has not been called for operator %d", op_index);
 	if (!cage_vertices || n_cage_vertices != r.n_cv) return fail(NSB_ERR_INVALID, "nsb_cage_deform: expected %u cage vertices", r.n_cv);
 	CU(cudaSetDevice(c->device));
 	cudaStream_t s = (cudaStream_t)stream_;
 	DevOp& d = c->h_ops[op_index];
 	const uint32_t n_cells = (uint32_t)NSB_GRID_CELLS, n_scan_blocks = (n_cells + SCAN_TILE - 1) / SCAN_TILE;
-	if (!r.d_counts) {
-		CU(cudaMalloc(&r.d_counts, (size_t)n_cells * 4));
-		CU(cudaMalloc(&r.d_block_sums, (size_t)n_scan_blocks * 4));
-		CU(cudaMalloc(&r.d_total, 4));
-		CU(cudaMalloc(&r.d_n_marks, 4));
-		CU(cudaMalloc(&r.d_boxes, 18 * sizeof(float)));
+	CU(r.d_counts.reserve(n_cells));
+	CU(r.d_block_sums.reserve(n_scan_blocks));
+	CU(r.d_total.reserve(1));
+	CU(r.d_n_marks.reserve(1));
+	if (!r.d_boxes.get()) {  // the scene aabb at [12..17] is either written or the boxes are not allocated
+		DevBuf<float> boxes;
+		CU(boxes.reserve(18));
 		float aabb[6] = {d.amin[0], d.amin[1], d.amin[2], d.amax[0], d.amax[1], d.amax[2]};
-		CU(cudaMemcpy(r.d_boxes + 12, aabb, sizeof(aabb), cudaMemcpyHostToDevice));
-		r.marks_cap = 1u << 20;
-		CU(cudaMalloc(&r.d_marks, (size_t)r.marks_cap * sizeof(Mark)));
+		CU(cudaMemcpy(boxes.get() + 12, aabb, sizeof(aabb), cudaMemcpyHostToDevice));
+		r.d_boxes = std::move(boxes);
 	}
-	float* d_verts = const_cast<float*>(d.verts);
+	CU(r.d_marks.reserve(1u << 20));
+	float* d_verts = r.verts.get();
 	const bool verbose = getenv("NSB_VERBOSE") != nullptr;
 	auto now = [] { timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return ts.tv_sec * 1e3 + ts.tv_nsec * 1e-6; };
 	const double t_start = now();
 	double t_marked = 0, t_launched = 0;
 	// 1. Cage::interpolate_with_mvc
-	CU(cudaMemcpyAsync(r.d_cage, cage_vertices, (size_t)3 * r.n_cv * sizeof(float), cudaMemcpyHostToDevice, s));
-	k_mvc_apply<<<(r.n_vertices + 127) / 128, 128, 3 * r.n_cv * sizeof(float), s>>>(r.d_mvc, r.n_vertices, r.n_cv, r.d_cage, d_verts);
+	CU(cudaMemcpyAsync(r.d_cage.get(), cage_vertices, (size_t)3 * r.n_cv * sizeof(float), cudaMemcpyHostToDevice, s));
+	k_mvc_apply<<<(r.n_vertices + 127) / 128, 128, 3 * r.n_cv * sizeof(float), s>>>(r.d_mvc.get(), r.n_vertices, r.n_cv, r.d_cage.get(), d_verts);
 	// 2. TetMesh::post_update_vertices, update_local_rotations
-	k_cage_bbox<<<1, 256, 0, s>>>(d_verts, r.n_vertices, r.d_boxes + 12, r.d_boxes);
-	if (d.rots) k_local_rotations<<<(d.n_tets + 63) / 64, 64, 0, s>>>(d_verts, d.orig_verts, d.tets, d.n_tets, const_cast<float*>(d.rots));
+	float* d_boxes = r.d_boxes.get();
+	k_cage_bbox<<<1, 256, 0, s>>>(d_verts, r.n_vertices, d_boxes + 12, d_boxes);
+	if (d.rots) k_local_rotations<<<(d.n_tets + 63) / 64, 64, 0, s>>>(d_verts, d.orig_verts, d.tets, d.n_tets, r.rots.get());
 	// 3. TetMesh::build_tet_grid: mark, scan, scatter, order
+	uint32_t* d_counts = r.d_counts.get();
+	unsigned int* d_n_marks = r.d_n_marks.get();
 	unsigned int n_marks = 0;
 	for (int attempt = 0; attempt < 2; ++attempt) {
-		CU(cudaMemsetAsync(r.d_counts, 0, (size_t)n_cells * 4, s));
-		CU(cudaMemsetAsync(r.d_n_marks, 0, 4, s));
-		k_tet_mark<<<d.n_tets * CASCADES, 128, 0, s>>>(d_verts, d.tets, d.n_tets, r.d_counts, r.d_marks, r.marks_cap, r.d_n_marks);
-		CU(cudaMemcpyAsync(&n_marks, r.d_n_marks, 4, cudaMemcpyDeviceToHost, s));
+		CU(cudaMemsetAsync(d_counts, 0, (size_t)n_cells * 4, s));
+		CU(cudaMemsetAsync(d_n_marks, 0, 4, s));
+		k_tet_mark<<<d.n_tets * CASCADES, 128, 0, s>>>(d_verts, d.tets, d.n_tets, d_counts, r.d_marks.get(), (uint32_t)r.d_marks.capacity(), d_n_marks);
+		CU(cudaMemcpyAsync(&n_marks, d_n_marks, 4, cudaMemcpyDeviceToHost, s));
 		CU(cudaStreamSynchronize(s));  // one sync per edit: the list length decides the allocation
 		t_marked = now();
-		if (n_marks <= r.marks_cap) break;
+		if (n_marks <= r.d_marks.capacity()) break;
 		if (attempt == 1) return fail(NSB_ERR_CUDA, "nsb_cage_deform: mark buffer overflow after regrow");
-		cudaFree(r.d_marks);
-		r.d_marks = nullptr;
-		r.marks_cap = n_marks + n_marks / 4;
-		CU(cudaMalloc(&r.d_marks, (size_t)r.marks_cap * sizeof(Mark)));
+		CU(r.d_marks.reserve((size_t)n_marks + n_marks / 4));
 	}
-	uint32_t* d_off = const_cast<uint32_t*>(d.lut_off);
-	k_scan_block_sums<<<n_scan_blocks, SCAN_THREADS, 0, s>>>(r.d_counts, n_cells, r.d_block_sums);
-	k_scan_sums<<<1, SCAN_THREADS, 0, s>>>(r.d_block_sums, n_scan_blocks, r.d_total);
-	k_scan_apply<<<n_scan_blocks, SCAN_THREADS, 0, s>>>(r.d_counts, n_cells, r.d_block_sums, r.d_total, d_off);
-	uint32_t* d_idx = const_cast<uint32_t*>(d.lut_idx);
-	if ((uint64_t)n_marks > r.idx_cap || !d_idx) {  // the list outgrew the array it lives in (uploaded or ours): take a larger one
-		cudaFree(r.d_idx);
-		r.d_idx = nullptr;
-		r.idx_cap = (uint64_t)n_marks + n_marks / 4 + 1;
-		CU(cudaMalloc(&r.d_idx, r.idx_cap * 4));
-		d_idx = r.d_idx;
-		d.lut_idx = r.d_idx;
+	// The list outgrew its array: take a larger one before the scan rewrites the offsets. No DevOp, on the host or on the device, points at
+	// a freed array: a failed allocation leaves the operator as it was, and the old list (in `idx` after the swap) lives past the DevOp upload.
+	DevBuf<uint32_t> idx;
+	if ((uint64_t)n_marks > r.lut_idx.capacity() || !r.lut_idx.get()) {
+		CU(idx.reserve((size_t)n_marks + n_marks / 4 + 1));
+		std::swap(r.lut_idx, idx);
+		d.lut_idx = r.lut_idx.get();
 	}
+	uint32_t* d_off = r.lut_off.get();
+	uint32_t* d_idx = r.lut_idx.get();
+	k_scan_block_sums<<<n_scan_blocks, SCAN_THREADS, 0, s>>>(d_counts, n_cells, r.d_block_sums.get());
+	k_scan_sums<<<1, SCAN_THREADS, 0, s>>>(r.d_block_sums.get(), n_scan_blocks, r.d_total.get());
+	k_scan_apply<<<n_scan_blocks, SCAN_THREADS, 0, s>>>(d_counts, n_cells, r.d_block_sums.get(), r.d_total.get(), d_off);
 	if (n_marks) {
-		k_tet_fill<<<(n_marks + 255) / 256, 256, 0, s>>>(r.d_marks, n_marks, d_off, r.d_counts, d_idx);
+		k_tet_fill<<<(n_marks + 255) / 256, 256, 0, s>>>(r.d_marks.get(), n_marks, d_off, d_counts, d_idx);
 		// the counts are all zero again and the marks are consumed: reuse them as the long-cell queue and the sort scratch
-		CU(cudaMemsetAsync(r.d_n_marks, 0, 4, s));
-		k_tet_sort<<<(n_cells + 255) / 256, 256, 0, s>>>(d_off, n_cells, d_idx, r.d_counts, r.d_n_marks);
-		k_tet_sort_long<<<c->sm_count * 4, 256, 0, s>>>(d_off, d_idx, r.d_counts, r.d_n_marks, reinterpret_cast<uint32_t*>(r.d_marks));
+		CU(cudaMemsetAsync(d_n_marks, 0, 4, s));
+		k_tet_sort<<<(n_cells + 255) / 256, 256, 0, s>>>(d_off, n_cells, d_idx, d_counts, d_n_marks);
+		k_tet_sort_long<<<c->sm_count * 4, 256, 0, s>>>(d_off, d_idx, d_counts, d_n_marks, reinterpret_cast<uint32_t*>(r.d_marks.get()));
 	}
 	r.n_idx = n_marks;
 	// 4. the operator's boxes and (possibly) its list pointer
 	float boxes[12];
 	t_launched = now();
-	CU(cudaMemcpyAsync(boxes, r.d_boxes, sizeof(boxes), cudaMemcpyDeviceToHost, s));
+	CU(cudaMemcpyAsync(boxes, d_boxes, sizeof(boxes), cudaMemcpyDeviceToHost, s));
 	CU(cudaStreamSynchronize(s));
 	if (verbose)
 		fprintf(stderr, "[nsb] cage_deform op %d: %u marks; mark phase %.3f ms, launches %.3f ms, drain %.3f ms\n", op_index, n_marks, t_marked - t_start,
 		        t_launched - t_marked, now() - t_launched);
 	cp3(d.bmin, boxes); cp3(d.bmax, boxes + 3); cp3(d.wbmin, boxes + 6); cp3(d.wbmax, boxes + 9);
-	CU(cudaMemcpyAsync(c->d_ops + op_index, &d, sizeof(DevOp), cudaMemcpyHostToDevice, s));
+	CU(cudaMemcpyAsync(c->d_ops.get() + op_index, &d, sizeof(DevOp), cudaMemcpyHostToDevice, s));
 	CU(cudaGetLastError());
 	return NSB_OK;
 }
@@ -1523,29 +1536,25 @@ extern "C" NsbStatus nsb_poisson_boundary(NsbContext* c, const float* points, ui
 	const uint32_t n = (uint32_t)n64, n_padded = next_multiple_u32(n, 128u);  // tcnn::batch_size_granularity (:2231)
 	std::vector<float> coords;
 	boundary_coords(points, n_points, p, coords);
-	float *d_coords = nullptr, *d_aabb = nullptr, *d_dens = nullptr, *d_shs = nullptr;
-	__half* d_net = nullptr;
-	auto cleanup = [&] { cudaFree(d_coords); cudaFree(d_aabb); cudaFree(d_dens); cudaFree(d_shs); cudaFree(d_net); };
-#define CUB_(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { cleanup(); return fail(NSB_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(e__)); } } while (0)
-	CUB_(cudaMalloc(&d_coords, (size_t)n * 7 * 4));
-	CUB_(cudaMalloc(&d_aabb, 6 * 4));
-	CUB_(cudaMalloc(&d_dens, (size_t)n_points * 4));
-	CUB_(cudaMalloc(&d_shs, (size_t)n_points * 27 * 4));
-	CUB_(cudaMalloc(&d_net, (size_t)16 * n_padded * 2));
-	CUB_(cudaMemcpy(d_coords, coords.data(), (size_t)n * 7 * 4, cudaMemcpyHostToDevice));
+	DevBuf<float> d_coords, d_aabb, d_dens, d_shs;
+	DevBuf<__half> d_net;
+	CU(d_coords.reserve((size_t)n * 7));
+	CU(d_aabb.reserve(6));
+	CU(d_dens.reserve(n_points));
+	CU(d_shs.reserve((size_t)n_points * 27));
+	CU(d_net.reserve((size_t)16 * n_padded));
+	CU(cudaMemcpy(d_coords.get(), coords.data(), (size_t)n * 7 * 4, cudaMemcpyHostToDevice));
 	float aabb[6] = {p->train_aabb_min[0], p->train_aabb_min[1], p->train_aabb_min[2], p->train_aabb_max[0], p->train_aabb_max[1], p->train_aabb_max[2]};
-	CUB_(cudaMemcpy(d_aabb, aabb, sizeof(aabb), cudaMemcpyHostToDevice));
+	CU(cudaMemcpy(d_aabb.get(), aabb, sizeof(aabb), cudaMemcpyHostToDevice));
 	uint32_t grid = n_padded / 128, cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
 	if (grid > cap) grid = cap;
-	(c->acc16 ? k_inference<false, true> : k_inference<false, false>)<<<grid, 128, sizeof(tc::TileSmem)>>>(c->model, d_coords, n, d_net, n_padded);  // inference_mixed_precision (:2286)
+	(c->acc16 ? k_inference<false, true> : k_inference<false, false>)<<<grid, 128, sizeof(tc::TileSmem)>>>(c->model, d_coords.get(), n, d_net.get(), n_padded);  // inference_mixed_precision (:2286)
 	const float scale = (float)(4 * M_PI / (double)n_sh);                                                // :2341
-	nsb::rebuild::k_boundary_fit<<<n_points, 32>>>(d_net, n_padded, d_coords, n_sh, p->rgb_activation, p->density_activation,
-	                                               p->is_inside ? c->d_bitfield : nullptr, d_aabb, scale, d_dens, d_shs);
-	CUB_(cudaGetLastError());
-	CUB_(cudaMemcpy(density_out, d_dens, (size_t)n_points * 4, cudaMemcpyDeviceToHost));
-	CUB_(cudaMemcpy(shs_out, d_shs, (size_t)n_points * 27 * 4, cudaMemcpyDeviceToHost));
-#undef CUB_
-	cleanup();
+	nsb::rebuild::k_boundary_fit<<<n_points, 32>>>(d_net.get(), n_padded, d_coords.get(), n_sh, p->rgb_activation, p->density_activation,
+	                                               p->is_inside ? c->d_bitfield.get() : nullptr, d_aabb.get(), scale, d_dens.get(), d_shs.get());
+	CU(cudaGetLastError());
+	CU(cudaMemcpy(density_out, d_dens.get(), (size_t)n_points * 4, cudaMemcpyDeviceToHost));
+	CU(cudaMemcpy(shs_out, d_shs.get(), (size_t)n_points * 27 * 4, cudaMemcpyDeviceToHost));
 	return NSB_OK;
 }
 extern "C" NsbStatus nsb_cage_set_membrane(NsbContext* c, int32_t op_index, const float* gamma, uint32_t n_cv, const float* inside_density,
@@ -1567,7 +1576,6 @@ extern "C" NsbStatus nsb_cage_set_membrane(NsbContext* c, int32_t op_index, cons
 		alpha_out[j] = a_out;
 		w_in[j] = (1.f < q) ? 1.f : q;  // std::min(alpha_in / alpha_out, 1.f)
 	}
-	float *d_gamma = nullptr, *d_small = nullptr;
 	const size_t small = (size_t)n_cv * (4 + 54);
 	std::vector<float> pack(small);
 	memcpy(pack.data(), alpha_out.data(), n_cv * 4);
@@ -1577,29 +1585,26 @@ extern "C" NsbStatus nsb_cage_set_membrane(NsbContext* c, int32_t op_index, cons
 	memcpy(pack.data() + 4 * (size_t)n_cv, inside_shs, (size_t)n_cv * 27 * 4);
 	memcpy(pack.data() + 31 * (size_t)n_cv, outside_shs, (size_t)n_cv * 27 * 4);
 	auto& r = c->rb[op_index];
-	if (r.mem_n_cv != n_cv) {  // scratch of the blend, kept with the operator (a host re-blends after every boundary re-sampling)
-		cudaFree(r.d_gamma); cudaFree(r.d_mem_small);
-		r.d_gamma = r.d_mem_small = nullptr;
-		CU(cudaMalloc(&r.d_gamma, (size_t)nv * n_cv * 4));
-		CU(cudaMalloc(&r.d_mem_small, small * 4));
-		r.mem_n_cv = n_cv;
-	}
-	d_gamma = r.d_gamma;
-	d_small = r.d_mem_small;
-	CU(cudaMemcpy(d_gamma, gamma, (size_t)nv * n_cv * 4, cudaMemcpyHostToDevice));
+	// scratch of the blend, kept with the operator (a host re-blends after every boundary re-sampling) and sized to its cage
+	if (r.d_mem_small.capacity() != small) { r.d_gamma = {}; r.d_mem_small = {}; }
+	CU(r.d_gamma.reserve((size_t)nv * n_cv));
+	CU(r.d_mem_small.reserve(small));
+	float* d_small = r.d_mem_small.get();
+	CU(cudaMemcpy(r.d_gamma.get(), gamma, (size_t)nv * n_cv * 4, cudaMemcpyHostToDevice));
 	CU(cudaMemcpy(d_small, pack.data(), small * 4, cudaMemcpyHostToDevice));
-	if (!d.shs) { void* q; CU(cudaMalloc(&q, (size_t)nv * 27 * 4)); c->op_allocs.push_back(q); d.shs = (const float*)q; }
-	if (!d.od) { void* q; CU(cudaMalloc(&q, (size_t)nv * 4)); c->op_allocs.push_back(q); d.od = (const float*)q; }
-	if (!d.rd) { void* q; CU(cudaMalloc(&q, (size_t)nv * 4)); c->op_allocs.push_back(q); d.rd = (const float*)q; }
+	// the boundary arrays, unless nsb_set_edit_ops uploaded them
+	CU(r.shs.reserve((size_t)nv * 27));
+	CU(r.od.reserve(nv));
+	CU(r.rd.reserve(nv));
+	d.shs = r.shs.get(); d.od = r.od.get(); d.rd = r.rd.get();
 	dim3 block(32, 4);
-	nsb::rebuild::k_membrane_blend<<<(nv + 3) / 4, block>>>(d_gamma, nv, n_cv, d_small, d_small + n_cv, d_small + 2 * (size_t)n_cv, d_small + 3 * (size_t)n_cv,
-	                                                        d_small + 4 * (size_t)n_cv, d_small + 31 * (size_t)n_cv, const_cast<float*>(d.shs),
-	                                                        const_cast<float*>(d.od), const_cast<float*>(d.rd));
+	nsb::rebuild::k_membrane_blend<<<(nv + 3) / 4, block>>>(r.d_gamma.get(), nv, n_cv, d_small, d_small + n_cv, d_small + 2 * (size_t)n_cv, d_small + 3 * (size_t)n_cv,
+	                                                        d_small + 4 * (size_t)n_cv, d_small + 31 * (size_t)n_cv, r.shs.get(), r.od.get(), r.rd.get());
 	CU(cudaGetLastError());
 	d.has_poisson_data = 1;
 	d.apply_poisson = apply_poisson ? 1 : 0;
 	d.amp = residual_amplitude;
-	CU(cudaMemcpy(c->d_ops + op_index, &d, sizeof(DevOp), cudaMemcpyHostToDevice));
+	CU(cudaMemcpy(c->d_ops.get() + op_index, &d, sizeof(DevOp), cudaMemcpyHostToDevice));
 	int any = 0;
 	for (const DevOp& o : c->h_ops) if (o.type == NSB_OP_CAGE && o.apply_poisson && o.has_poisson_data && o.n_tets) any = 1;
 	c->any_poisson = any;
@@ -1729,37 +1734,35 @@ extern "C" NsbStatus nsb_render(NsbContext* c, const NsbFrame* frame, float* fb_
 	uint32_t n_tiles = (uint32_t)(f.tiles_x * f.tiles_y);
 	uint32_t my_tiles = (n_tiles + (uint32_t)f.tile_world - 1 - (uint32_t)f.tile_rank) / (uint32_t)f.tile_world;
 	size_t n_local = (size_t)my_tiles * TILE_PIXELS;
-	if (n_local > c->list_capacity) {
+	if (n_local > c->d_list.capacity()) {
 		CU(cudaStreamSynchronize(stream));
-		cudaFree(c->d_list);
-		c->d_list = nullptr; c->list_capacity = 0;
-		CU(cudaMalloc(&c->d_list, n_local * sizeof(RayRec)));
-		c->list_capacity = n_local;
+		CU(c->d_list.reserve(n_local));
 	}
 	// frames whose ray generation is not the pinhole fast path (ABI 3): k_prepare_rays<true>; with a general camera the rays travel in a side buffer
 	const bool general = f.general_camera || f.envmap != nullptr || f.mode == NSB_RENDER_DISTORTION;
 	float* ray_od = nullptr;
 	if (f.general_camera) {
-		if (n_local > c->ray_od_capacity) {
+		if (n_local * 6 > c->d_ray_od.capacity()) {
 			CU(cudaStreamSynchronize(stream));
-			cudaFree(c->d_ray_od);
-			c->d_ray_od = nullptr; c->ray_od_capacity = 0;
-			CU(cudaMalloc(&c->d_ray_od, n_local * 6 * sizeof(float)));
-			c->ray_od_capacity = n_local;
+			CU(c->d_ray_od.reserve(n_local * 6));
 		}
-		ray_od = c->d_ray_od;
+		ray_od = c->d_ray_od.get();
 	}
+	const uint8_t* bitfield = c->has_occ ? c->d_bitfield.get() : nullptr;
+	RayRec* list = c->d_list.get();
+	uint32_t* counters = c->d_counters.get();
+	unsigned long long* stats = c->d_stats.get();
 	CU(cudaEventRecord(c->ev0, stream));
 	CU(cudaEventRecord(c->evm, stream));
-	CU(cudaMemsetAsync(c->d_counters, 0, 2 * sizeof(uint32_t), stream));
-	CU(cudaMemsetAsync(c->d_stats, 0, ST_N * sizeof(unsigned long long), stream));
+	CU(cudaMemsetAsync(counters, 0, 2 * sizeof(uint32_t), stream));
+	CU(cudaMemsetAsync(stats, 0, ST_N * sizeof(unsigned long long), stream));
 	if (n_local > 0) {
 		if (general)
-			k_prepare_rays<true><<<(unsigned)((n_local + 255) / 256), 256, 0, stream>>>(f, c->has_occ ? c->d_bitfield : nullptr, reinterpret_cast<float4*>(fb_dev), depth_dev, c->d_list,
-			                                                                         ray_od, c->d_counters, (uint32_t)n_local, c->d_stats);
+			k_prepare_rays<true><<<(unsigned)((n_local + 255) / 256), 256, 0, stream>>>(f, bitfield, reinterpret_cast<float4*>(fb_dev), depth_dev, list, ray_od, counters,
+			                                                                         (uint32_t)n_local, stats);
 		else
-			k_prepare_rays<false><<<(unsigned)((n_local + 255) / 256), 256, 0, stream>>>(f, c->has_occ ? c->d_bitfield : nullptr, reinterpret_cast<float4*>(fb_dev), depth_dev, c->d_list,
-			                                                                          nullptr, c->d_counters, (uint32_t)n_local, c->d_stats);
+			k_prepare_rays<false><<<(unsigned)((n_local + 255) / 256), 256, 0, stream>>>(f, bitfield, reinterpret_cast<float4*>(fb_dev), depth_dev, list, nullptr, counters,
+			                                                                          (uint32_t)n_local, stats);
 		CU(cudaGetLastError());
 		CU(cudaEventRecord(c->evm, stream));
 		const bool ops_on = f.apply_ops && c->n_ops > 0;
@@ -1767,8 +1770,8 @@ extern "C" NsbStatus nsb_render(NsbContext* c, const NsbFrame* frame, float* fb_
 		uint32_t grid = (uint32_t)c->sm_count;  // one CTA per SM
 		if (grid > (my_tiles + tiles - 1) / tiles) grid = (my_tiles + tiles - 1) / tiles;
 		auto kernel = ops_on ? (c->acc16 ? k_render_fused<true, true> : k_render_fused<true, false>) : (c->acc16 ? k_render_fused<false, true> : k_render_fused<false, false>);
-		kernel<<<grid, 128 * tiles, ops_on ? sizeof(RenderSmemT<render_tiles(true)>) : sizeof(RenderSmemT<render_tiles(false)>), stream>>>(f, c->model, c->has_occ ? c->d_bitfield : nullptr, c->d_ops, c->n_ops, c->any_poisson,
-		                                                          reinterpret_cast<float4*>(fb_dev), depth_dev, c->d_list, ray_od, c->d_counters, c->d_counters + 1, c->d_stats);
+		kernel<<<grid, 128 * tiles, ops_on ? sizeof(RenderSmemT<render_tiles(true)>) : sizeof(RenderSmemT<render_tiles(false)>), stream>>>(f, c->model, bitfield, c->d_ops.get(), c->n_ops, c->any_poisson,
+		                                                          reinterpret_cast<float4*>(fb_dev), depth_dev, list, ray_od, counters, counters + 1, stats);
 		CU(cudaGetLastError());
 	}
 	CU(cudaEventRecord(c->ev1, stream));
@@ -1782,19 +1785,16 @@ extern "C" NsbStatus nsb_render_host(NsbContext* c, const NsbFrame* frame, float
 	CU(cudaSetDevice(c->device));
 	size_t n = (size_t)frame->width * (size_t)frame->height;
 	if (n == 0) return fail(NSB_ERR_INVALID, "empty frame");
-	if (n > c->fb_pixels) {
-		cudaFree(c->d_fb); cudaFree(c->d_depth);
-		c->d_fb = nullptr; c->d_depth = nullptr; c->fb_pixels = 0;
-		CU(cudaMalloc(&c->d_fb, n * 16));
-		CU(cudaMalloc(&c->d_depth, n * 4));
-		c->fb_pixels = n;
-	}
-	CU(cudaMemsetAsync(c->d_fb, 0, n * 16, c->stream));  // render_buffer.clear_frame (testbed.cu:2635)
-	CU(cudaMemsetAsync(c->d_depth, 0, n * 4, c->stream));
-	NsbStatus st = nsb_render(c, frame, c->d_fb, c->d_depth, c->stream);
+	CU(c->d_fb.reserve(n * 4));
+	CU(c->d_depth.reserve(n));
+	float* fb = c->d_fb.get();
+	float* depth = c->d_depth.get();
+	CU(cudaMemsetAsync(fb, 0, n * 16, c->stream));  // render_buffer.clear_frame (testbed.cu:2635)
+	CU(cudaMemsetAsync(depth, 0, n * 4, c->stream));
+	NsbStatus st = nsb_render(c, frame, fb, depth, c->stream);
 	if (st != NSB_OK) return st;
-	CU(cudaMemcpyAsync(fb_host, c->d_fb, n * 16, cudaMemcpyDeviceToHost, c->stream));
-	if (depth_host) CU(cudaMemcpyAsync(depth_host, c->d_depth, n * 4, cudaMemcpyDeviceToHost, c->stream));
+	CU(cudaMemcpyAsync(fb_host, fb, n * 16, cudaMemcpyDeviceToHost, c->stream));
+	if (depth_host) CU(cudaMemcpyAsync(depth_host, depth, n * 4, cudaMemcpyDeviceToHost, c->stream));
 	CU(cudaStreamSynchronize(c->stream));
 	return NSB_OK;
 }
@@ -1804,30 +1804,26 @@ extern "C" NsbStatus nsb_render_host_async(NsbContext* c, const NsbFrame* frame,
 	CU(cudaSetDevice(c->device));
 	const size_t n = (size_t)frame->width * (size_t)frame->height;
 	if (n == 0) return fail(NSB_ERR_INVALID, "empty frame");
-	if (n > c->fb2_pixels) {
+	if (c->d_fb2[0].capacity() < n * 4 || c->d_fb2[1].capacity() < n * 4 || c->d_depth2[0].capacity() < n || c->d_depth2[1].capacity() < n) {
 		CU(cudaStreamSynchronize(c->stream));
 		CU(cudaStreamSynchronize(c->copy_stream));
 		for (int i = 0; i < 2; ++i) {
-			cudaFree(c->d_fb2[i]); cudaFree(c->d_depth2[i]);
-			c->d_fb2[i] = nullptr; c->d_depth2[i] = nullptr;
+			CU(c->d_fb2[i].reserve(n * 4));
+			CU(c->d_depth2[i].reserve(n));
 		}
-		c->fb2_pixels = 0;
-		for (int i = 0; i < 2; ++i) {
-			CU(cudaMalloc(&c->d_fb2[i], n * 16));
-			CU(cudaMalloc(&c->d_depth2[i], n * 4));
-		}
-		c->fb2_pixels = n;
 	}
 	const int slot = (int)(c->host_seq & 1u);
+	float* fb = c->d_fb2[slot].get();
+	float* depth = c->d_depth2[slot].get();
 	if (c->host_seq >= 2) CU(cudaStreamWaitEvent(c->stream, c->copy_done[slot], 0));  // the copy that last read this slot (two tickets ago)
-	CU(cudaMemsetAsync(c->d_fb2[slot], 0, n * 16, c->stream));  // render_buffer.clear_frame (testbed.cu:2635)
-	CU(cudaMemsetAsync(c->d_depth2[slot], 0, n * 4, c->stream));
-	NsbStatus st = nsb_render(c, frame, c->d_fb2[slot], c->d_depth2[slot], c->stream);
+	CU(cudaMemsetAsync(fb, 0, n * 16, c->stream));  // render_buffer.clear_frame (testbed.cu:2635)
+	CU(cudaMemsetAsync(depth, 0, n * 4, c->stream));
+	NsbStatus st = nsb_render(c, frame, fb, depth, c->stream);
 	if (st != NSB_OK) return st;
 	CU(cudaEventRecord(c->render_done[slot], c->stream));
 	CU(cudaStreamWaitEvent(c->copy_stream, c->render_done[slot], 0));
-	CU(cudaMemcpyAsync(fb_host, c->d_fb2[slot], n * 16, cudaMemcpyDeviceToHost, c->copy_stream));
-	if (depth_host) CU(cudaMemcpyAsync(depth_host, c->d_depth2[slot], n * 4, cudaMemcpyDeviceToHost, c->copy_stream));
+	CU(cudaMemcpyAsync(fb_host, fb, n * 16, cudaMemcpyDeviceToHost, c->copy_stream));
+	if (depth_host) CU(cudaMemcpyAsync(depth_host, depth, n * 4, cudaMemcpyDeviceToHost, c->copy_stream));
 	CU(cudaEventRecord(c->copy_done[slot], c->copy_stream));
 	*ticket = c->host_seq++;
 	return NSB_OK;
@@ -1855,7 +1851,7 @@ extern "C" NsbStatus nsb_get_stats(NsbContext* c, NsbRenderStats* out) {
 	if (!c->timed) return NSB_OK;
 	CU(cudaEventSynchronize(c->ev1));
 	unsigned long long h[ST_N];
-	CU(cudaMemcpy(h, c->d_stats, sizeof(h), cudaMemcpyDeviceToHost));
+	CU(cudaMemcpy(h, c->d_stats.get(), sizeof(h), cudaMemcpyDeviceToHost));
 	out->n_rays = h[ST_RAYS]; out->n_rays_alive = h[ST_ALIVE]; out->n_hit = h[ST_HIT]; out->n_samples = h[ST_SAMPLES]; out->n_old_samples = h[ST_OLD];
 	out->n_kernel_launches = c->launches;
 	CU(cudaEventElapsedTime(&out->gpu_ms, c->ev0, c->ev1));
@@ -1870,7 +1866,7 @@ extern "C" NsbStatus nsb_debug_counters(NsbContext* c, uint64_t* out, int32_t n)
 	CU(cudaSetDevice(c->device));
 	if (c->timed) CU(cudaEventSynchronize(c->ev1));
 	unsigned long long h[ST_N];
-	CU(cudaMemcpy(h, c->d_stats, sizeof(h), cudaMemcpyDeviceToHost));
+	CU(cudaMemcpy(h, c->d_stats.get(), sizeof(h), cudaMemcpyDeviceToHost));
 	for (int i = 0; i < 7; ++i) out[i] = h[ST_ROUNDS + i];
 	return NSB_OK;
 }
@@ -1974,7 +1970,7 @@ extern "C" NsbStatus nsb_encode(NsbContext* c, const float* coords, uint32_t n, 
 // op_index >= 0: that operator alone = one EditOperator virtual call (outputs are not cleared, as the virtuals do not clear them)
 static NsbStatus op_range(NsbContext* c, int32_t op_index, const DevOp** ops, int* n_ops) {
 	if (op_index >= c->n_ops) return fail(NSB_ERR_INVALID, "operator %d of %d", op_index, c->n_ops);
-	*ops = op_index < 0 ? c->d_ops : c->d_ops + op_index;
+	*ops = op_index < 0 ? c->d_ops.get() : c->d_ops.get() + op_index;
 	*n_ops = op_index < 0 ? c->n_ops : 1;
 	return NSB_OK;
 }
@@ -2044,8 +2040,9 @@ extern "C" NsbStatus nsb_march_trace(NsbContext* c, const NsbFrame* frame, const
 	if (st != NSB_OK) return st;
 	if (n_pixels == 0) return NSB_OK;
 	CU(cudaSetDevice(c->device));
-	if (f.general_camera) k_march_trace<true><<<(n_pixels + 63) / 64, 64, 0, (cudaStream_t)stream>>>(f, c->has_occ ? c->d_bitfield : nullptr, pixels, n_pixels, max_samples, rec, idx, count);
-	else k_march_trace<false><<<(n_pixels + 63) / 64, 64, 0, (cudaStream_t)stream>>>(f, c->has_occ ? c->d_bitfield : nullptr, pixels, n_pixels, max_samples, rec, idx, count);
+	const uint8_t* bitfield = c->has_occ ? c->d_bitfield.get() : nullptr;
+	if (f.general_camera) k_march_trace<true><<<(n_pixels + 63) / 64, 64, 0, (cudaStream_t)stream>>>(f, bitfield, pixels, n_pixels, max_samples, rec, idx, count);
+	else k_march_trace<false><<<(n_pixels + 63) / 64, 64, 0, (cudaStream_t)stream>>>(f, bitfield, pixels, n_pixels, max_samples, rec, idx, count);
 	CU(cudaGetLastError());
 	return NSB_OK;
 }
