@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define NSB_ABI_VERSION 3
+#define NSB_ABI_VERSION 4
 
 /* reference: common_nerf.h:16-39 */
 #define NSB_NERF_GRIDSIZE 128u
@@ -415,6 +415,36 @@ NsbStatus nsb_interpolate_with_mvc(const float* weights, uint32_t n_points, uint
                                    const float* cage_vertices, float* points_out);
 /* replaces TetMesh::update_local_rotations (tet_mesh.cu:38-74): rotations [9*n_tets] column-major. */
 NsbStatus nsb_local_rotations(const float* vertices, const float* original_vertices, const uint32_t* tets, uint32_t n_tets, float* rotations);
+
+/* ---- mesh extraction (ABI 4): Testbed::marching_cubes (testbed_nerf.cu:4614-4649), as the GUI's "Mesh it!" (testbed.cu:932-942),
+ * compute_marching_cubes_mesh (python_api.cu:105-126) and compute_and_save_marching_cubes_mesh (testbed.cu:337-343) run it ---------- */
+typedef struct {
+	int32_t res[3];                               /* grid points per axis: positive multiples of 16 (testbed_nerf.cu:4615-4617) */
+	float   aabb_min[3], aabb_max[3];             /* the box sampled (m_render_aabb by default) */
+	float   train_aabb_min[3], train_aabb_max[3]; /* m_aabb */
+} NsbGridQuery;
+/* replaces Testbed::get_density_on_grid (testbed_nerf.cu:4538-4586) in NeRF mode: density_dev (DEVICE float[res_x*res_y*res_z], x fastest)
+ * receives float(raw fp16 density output) at aabb_min + (x/res_x, y/res_y, z/res_z) * (aabb_max - aabb_min), or -10000 where the context's
+ * running density grid (Testbed::Nerf::density_grid) is below NERF_MIN_OPTICAL_THICKNESS at that position (grid_samples_half_to_float :465-481).
+ * NSB_ERR_STATE without a model or a density grid. Stream-ordered. */
+NsbStatus nsb_density_on_grid(NsbContext* ctx, const NsbGridQuery* query, float* density_dev, void* stream);
+/* replaces marching_cubes_gpu (marching_cubes.cu:730-758) on any DEVICE float grid (x fastest; e.g. the output above, or
+ * GrowingSelection::extract_fine_mesh's 0/1 selection grid, growing_selection.cu:2096-2162): builds the mesh into arrays the context owns.
+ * Vertices are the reference's edge crossings bit for bit (gen_vertices :217-265), ordered by (grid point, axis x, y, z); triangles by
+ * (cell, table order) with the table of nsb_mc_table.h, so two calls give the same arrays. *n_vertices, *n_indices: exact counts.
+ * Synchronises the stream once, for the counts. Scratch: 4 B per grid point. */
+NsbStatus nsb_marching_cubes(NsbContext* ctx, const float* density_dev, const int32_t res[3], const float aabb_min[3], const float aabb_max[3], float thresh,
+                             uint64_t* n_vertices, uint64_t* n_indices, void* stream);
+/* replaces compute_mesh_1ring's normals (marching_cubes.cu:656-662, accumulate_1ring :267-302) and Testbed::compute_mesh_vertex_colors
+ * (testbed_nerf.cu:4515-4536) for the last nsb_marching_cubes mesh: normal = sum of (pb-pa)x(pa-pc) over the vertex's triangles in
+ * triangle order (not normalised, like m_mesh.vert_normals); colour = the network at the vertex, direction normalize(pos - 0.5),
+ * through network_to_rgb and, when linear_colors, linear_to_srgb (extract_srgb_with_activation :338-351). Stream-ordered. */
+NsbStatus nsb_mesh_shade(NsbContext* ctx, const float train_aabb_min[3], const float train_aabb_max[3], int32_t rgb_activation, int32_t linear_colors, void* stream);
+/* Copies the mesh back (HOST pointers, any may be NULL; synchronises the device). vertices / normals / colors: [3 * vertex_rows];
+ * vertex_rows may be up to n_vertices rounded up to 128, the reference's row count (marching_cubes.cu:751-753): the padding rows are
+ * at the origin with a zero normal and the network's colour there. indices: [index_capacity >= n_indices]. */
+NsbStatus nsb_mesh_download(NsbContext* ctx, float* vertices, float* normals, float* colors, uint64_t vertex_rows, uint32_t* indices,
+                            uint64_t index_capacity);
 
 #ifdef __cplusplus
 }

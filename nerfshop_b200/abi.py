@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libnerfshop_b200.so")
 
-NSB_ABI_VERSION = 3
+NSB_ABI_VERSION = 4
 NSB_MLP_ACC_F32, NSB_MLP_ACC_F16 = 0, 1
 NSB_NERF_GRIDSIZE = 128
 NSB_NERF_CASCADES = 5
@@ -125,6 +125,11 @@ class NsbRenderStats(C.Structure):
     ]
 
 
+class NsbGridQuery(C.Structure):
+    """Arguments of Testbed::get_density_on_grid (testbed_nerf.cu:4538-4586) in NeRF mode."""
+    _fields_ = [("res", i32 * 3), ("aabb_min", f32 * 3), ("aabb_max", f32 * 3), ("train_aabb_min", f32 * 3), ("train_aabb_max", f32 * 3)]
+
+
 # every symbol include/nerfshop_b200.h declares (tests/test_abi.py checks the .so exports all of them)
 EXPORTED_SYMBOLS = [
     "nsb_abi_version", "nsb_last_error", "nsb_create", "nsb_destroy",
@@ -136,6 +141,7 @@ EXPORTED_SYMBOLS = [
     "nsb_inference", "nsb_density", "nsb_encode", "nsb_map_rays", "nsb_poisson_residuals", "nsb_map_rays_op", "nsb_poisson_residuals_op",
     "nsb_map_positions", "nsb_poisson_residual_density", "nsb_march_trace",
     "nsb_build_tet_grid", "nsb_compute_mvc", "nsb_interpolate_with_mvc", "nsb_local_rotations",
+    "nsb_density_on_grid", "nsb_marching_cubes", "nsb_mesh_shade", "nsb_mesh_download",
 ]
 
 _lib = None
@@ -205,6 +211,10 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.nsb_compute_mvc.argtypes = [vp, u32, vp, u32, vp, u32, f32, vp]
     lib.nsb_interpolate_with_mvc.argtypes = [vp, u32, u32, vp, vp]
     lib.nsb_local_rotations.argtypes = [vp, vp, vp, u32, vp]
+    lib.nsb_density_on_grid.argtypes = [vp, C.POINTER(NsbGridQuery), vp, vp]
+    lib.nsb_marching_cubes.argtypes = [vp, vp, C.POINTER(i32), C.POINTER(f32), C.POINTER(f32), f32, C.POINTER(u64), C.POINTER(u64), vp]
+    lib.nsb_mesh_shade.argtypes = [vp, C.POINTER(f32), C.POINTER(f32), i32, i32, vp]
+    lib.nsb_mesh_download.argtypes = [vp, vp, vp, vp, u64, vp, u64]
     for name in EXPORTED_SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("nsb_last_error", "nsb_abi_version"):

@@ -918,6 +918,8 @@ __global__ void k_unpack_gathered(const float4* __restrict__ gathered, const flo
 	if (depth && gathered_depth) depth[p] = gathered_depth[(size_t)rank * rank_stride + q];
 }
 
+#include "nsb_mesh.cuh"
+
 // =====================================================================================================
 // host side: context, uploads, C ABI
 // =====================================================================================================
@@ -1014,6 +1016,16 @@ struct NsbContext {
 	cudaStream_t copy_stream = nullptr;
 	cudaEvent_t render_done[2] = {nullptr, nullptr}, copy_done[2] = {nullptr, nullptr};
 	uint64_t host_seq = 0;  // tickets issued
+	// the mesh of nsb_marching_cubes (Testbed::m_mesh): vertex rows = n_vertices rounded up to 128 like marching_cubes.cu:751-753, the padding
+	// rows at the origin; normals and colours are written by nsb_mesh_shade
+	DevBuf<float> mesh_verts, mesh_normals, mesh_colors;
+	DevBuf<uint32_t> mesh_idx;
+	uint64_t mesh_nv = 0, mesh_ni = 0;
+	bool has_mesh = false, mesh_shaded = false;
+	DevBuf<uint32_t> mc_voff, mc_tiles;  // first vertex id per grid point (4 B per point), per-tile vertex and triangle offsets
+	DevBuf<unsigned long long> mc_totals;
+	DevBuf<uint32_t> mesh_start, mesh_cursor, mesh_adj;  // per-vertex triangle lists of nsb_mesh_shade
+	DevBuf<uint8_t> mesh_scan_tmp;
 
 	~NsbContext() {  // the device arrays free themselves
 		for (cudaEvent_t e : {ev0, ev1, evm, render_done[0], render_done[1], copy_done[0], copy_done[1]}) if (e) cudaEventDestroy(e);
@@ -1128,6 +1140,9 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 		CU(set_smem((const void*)k_inference<true, true>, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
 		CU(set_smem((const void*)k_density_grid_update<false>, sizeof(tc::TileSmem), c->grid_update_ctas_per_sm));
 		CU(set_smem((const void*)k_density_grid_update<true>, sizeof(tc::TileSmem), c->grid_update_ctas_per_sm));
+		for (const void* f : {(const void*)mesh::k_density_on_grid<false>, (const void*)mesh::k_density_on_grid<true>, (const void*)mesh::k_mesh_colors<false>,
+		                      (const void*)mesh::k_mesh_colors<true>})
+			CU(set_smem(f, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
 	}
 	if (getenv("NSB_VERBOSE"))
 		fprintf(stderr, "[nsb] device %d: %d SMs; k_render_fused %d tiles/CTA (%d with operators), %d regs, %zu B smem; inference %d CTAs/SM, grid update %d CTAs/SM\n", device, c->sm_count,
@@ -2044,5 +2059,141 @@ extern "C" NsbStatus nsb_march_trace(NsbContext* c, const NsbFrame* frame, const
 	if (f.general_camera) k_march_trace<true><<<(n_pixels + 63) / 64, 64, 0, (cudaStream_t)stream>>>(f, bitfield, pixels, n_pixels, max_samples, rec, idx, count);
 	else k_march_trace<false><<<(n_pixels + 63) / 64, 64, 0, (cudaStream_t)stream>>>(f, bitfield, pixels, n_pixels, max_samples, rec, idx, count);
 	CU(cudaGetLastError());
+	return NSB_OK;
+}
+
+// ---- mesh extraction (Testbed::marching_cubes, testbed_nerf.cu:4614-4649) -------------------------------------------------
+static bool grid_res_ok(const int32_t* res) {  // positive multiples of 16 (testbed_nerf.cu:4615-4617) whose point count, padded to 128, fits 32 bits
+	for (int a = 0; a < 3; ++a)
+		if (res[a] <= 0 || res[a] % 16 != 0) return false;
+	return (uint64_t)res[0] * (uint64_t)res[1] * (uint64_t)res[2] <= 0xffffffffull - 127ull;
+}
+
+extern "C" NsbStatus nsb_density_on_grid(NsbContext* c, const NsbGridQuery* q, float* density_dev, void* stream) {
+	if (!c || !q || !density_dev) return fail(NSB_ERR_INVALID, "null argument");
+	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_density_on_grid: nsb_upload_model has not been called");
+	if (!c->d_density_grid.get()) return fail(NSB_ERR_STATE, "nsb_density_on_grid: no density grid (nsb_upload_density_grid or nsb_update_density_grid)");
+	if (!grid_res_ok(q->res)) return fail(NSB_ERR_INVALID, "nsb_density_on_grid: res must be positive multiples of 16 with a 32-bit point count");
+	CU(cudaSetDevice(c->device));
+	mesh::GridQuery g;
+	for (int a = 0; a < 3; ++a) {
+		g.res[a] = (uint32_t)q->res[a];
+		g.inv_res[a] = 1.0f / (float)q->res[a];
+		g.rmin[a] = q->aabb_min[a];
+		g.rext[a] = q->aabb_max[a] - q->aabb_min[a];
+		g.tmin[a] = q->train_aabb_min[a];
+		g.tmax[a] = q->train_aabb_max[a];
+	}
+	const uint32_t n_padded = next_multiple_u32(g.res[0] * g.res[1] * g.res[2], 128u);
+	uint32_t grid = n_padded / 128;
+	const uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
+	if (grid > cap) grid = cap;
+	(c->acc16 ? mesh::k_density_on_grid<true> : mesh::k_density_on_grid<false>)<<<grid, 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(
+		c->model, g, c->d_density_grid.get(), density_dev);
+	CU(cudaGetLastError());
+	return NSB_OK;
+}
+
+extern "C" NsbStatus nsb_marching_cubes(NsbContext* c, const float* density_dev, const int32_t* res, const float* aabb_min, const float* aabb_max, float thresh,
+                                        uint64_t* n_vertices, uint64_t* n_indices, void* stream_) {
+	if (!c || !density_dev || !res || !aabb_min || !aabb_max) return fail(NSB_ERR_INVALID, "null argument");
+	if (!grid_res_ok(res)) return fail(NSB_ERR_INVALID, "nsb_marching_cubes: res must be positive multiples of 16 with a 32-bit point count");
+	CU(cudaSetDevice(c->device));
+	cudaStream_t st = (cudaStream_t)stream_;
+	c->has_mesh = c->mesh_shaded = false;
+	c->mesh_nv = c->mesh_ni = 0;
+	mesh::McGrid g;
+	g.d = density_dev;
+	g.rx = (uint32_t)res[0]; g.ry = (uint32_t)res[1]; g.rz = (uint32_t)res[2];
+	g.rxy = g.rx * g.ry;
+	g.n = g.rxy * g.rz;
+	g.thresh = thresh;
+	const uint32_t n_tiles = (g.n + mesh::TILE - 1) / mesh::TILE;
+	CU(c->mc_tiles.reserve(2 * (size_t)n_tiles));
+	CU(c->mc_voff.reserve(g.n));
+	CU(c->mc_totals.reserve(2));
+	uint32_t* tile_nv = c->mc_tiles.get();
+	uint32_t* tile_nt = c->mc_tiles.get() + n_tiles;
+	mesh::k_mc_count<<<n_tiles, mesh::THREADS, 0, st>>>(g, tile_nv, tile_nt);
+	mesh::k_mc_scan<<<1, 512, 0, st>>>(n_tiles, tile_nv, tile_nt, c->mc_totals.get());
+	CU(cudaGetLastError());
+	unsigned long long tot[2];
+	CU(cudaMemcpyAsync(tot, c->mc_totals.get(), sizeof(tot), cudaMemcpyDeviceToHost, st));
+	CU(cudaStreamSynchronize(st));  // the one synchronisation: the sizes of the outputs (marching_cubes.cu:747-749)
+	const uint64_t rows = (tot[0] + 127ull) & ~127ull;
+	if (rows > 0xffffffffull || 3ull * tot[1] > 0xffffffffull)
+		return fail(NSB_ERR_INVALID, "nsb_marching_cubes: %llu vertices / %llu triangles do not fit 32-bit indices", tot[0], tot[1]);
+	CU(c->mesh_verts.reserve(3 * rows));
+	CU(c->mesh_idx.reserve(3 * tot[1]));
+	if (rows) CU(cudaMemsetAsync(c->mesh_verts.get(), 0, 3 * rows * sizeof(float), st));  // verts_out.memset(0): the padding rows sit at the origin
+	float sc[3];
+	for (int a = 0; a < 3; ++a) sc[a] = (aabb_max[a] - aabb_min[a]) / (float)res[a];  // (aabb.max - aabb.min).cwiseQuotient(res_3d) (:224)
+	mesh::k_mc_vertices<<<n_tiles, mesh::THREADS, 0, st>>>(g, tile_nv, sc[0], sc[1], sc[2], aabb_min[0], aabb_min[1], aabb_min[2], c->mc_voff.get(), c->mesh_verts.get());
+	mesh::k_mc_faces<<<n_tiles, mesh::THREADS, 0, st>>>(g, tile_nt, c->mc_voff.get(), c->mesh_idx.get());
+	CU(cudaGetLastError());
+	c->mesh_nv = tot[0];
+	c->mesh_ni = 3 * tot[1];
+	c->has_mesh = true;
+	if (n_vertices) *n_vertices = c->mesh_nv;
+	if (n_indices) *n_indices = c->mesh_ni;
+	return NSB_OK;
+}
+
+extern "C" NsbStatus nsb_mesh_shade(NsbContext* c, const float* train_aabb_min, const float* train_aabb_max, int32_t rgb_activation, int32_t linear_colors, void* stream_) {
+	if (!c || !train_aabb_min || !train_aabb_max) return fail(NSB_ERR_INVALID, "null argument");
+	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_mesh_shade: nsb_upload_model has not been called");
+	if (!c->has_mesh) return fail(NSB_ERR_STATE, "nsb_mesh_shade: no mesh (nsb_marching_cubes)");
+	if (rgb_activation < NSB_ACT_NONE || rgb_activation > NSB_ACT_EXPONENTIAL) return fail(NSB_ERR_INVALID, "nsb_mesh_shade: bad rgb_activation");
+	CU(cudaSetDevice(c->device));
+	cudaStream_t st = (cudaStream_t)stream_;
+	const uint32_t nv = (uint32_t)c->mesh_nv, rows = (uint32_t)((c->mesh_nv + 127ull) & ~127ull), nt = (uint32_t)(c->mesh_ni / 3);
+	c->mesh_shaded = false;
+	if (rows == 0) { c->mesh_shaded = true; return NSB_OK; }
+	CU(c->mesh_normals.reserve(3 * (size_t)rows));
+	CU(c->mesh_colors.reserve(3 * (size_t)rows));
+	CU(c->mesh_start.reserve((size_t)nv + 1));
+	CU(c->mesh_cursor.reserve((size_t)nv + 1));
+	CU(c->mesh_adj.reserve(nt ? (size_t)3 * nt : 1));
+	size_t tmp_bytes = 0;
+	CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, c->mesh_cursor.get(), c->mesh_start.get(), nv + 1, st));
+	CU(c->mesh_scan_tmp.reserve(tmp_bytes));
+	CU(cudaMemsetAsync(c->mesh_cursor.get(), 0, ((size_t)nv + 1) * 4, st));
+	if (nt) mesh::k_mesh_degree<<<(nt + 255) / 256, 256, 0, st>>>(nt, c->mesh_idx.get(), c->mesh_cursor.get());
+	CU(cub::DeviceScan::ExclusiveSum(c->mesh_scan_tmp.get(), tmp_bytes, c->mesh_cursor.get(), c->mesh_start.get(), nv + 1, st));
+	CU(cudaMemsetAsync(c->mesh_cursor.get(), 0, ((size_t)nv + 1) * 4, st));
+	if (nt) mesh::k_mesh_fill<<<(nt + 255) / 256, 256, 0, st>>>(nt, c->mesh_idx.get(), c->mesh_start.get(), c->mesh_cursor.get(), c->mesh_adj.get());
+	mesh::k_mesh_normals<<<(rows + 255) / 256, 256, 0, st>>>(nv, rows, c->mesh_verts.get(), c->mesh_idx.get(), c->mesh_start.get(), c->mesh_adj.get(),
+	                                                        c->mesh_normals.get());
+	mesh::Aabb train;
+	for (int a = 0; a < 3; ++a) { train.mn[a] = train_aabb_min[a]; train.mx[a] = train_aabb_max[a]; }
+	uint32_t grid = rows / 128;
+	const uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
+	if (grid > cap) grid = cap;
+	(c->acc16 ? mesh::k_mesh_colors<true> : mesh::k_mesh_colors<false>)<<<grid, 128, sizeof(tc::TileSmem), st>>>(
+		c->model, rows, c->mesh_verts.get(), train, rgb_activation, linear_colors ? 1 : 0, c->mesh_colors.get());
+	CU(cudaGetLastError());
+	c->mesh_shaded = true;
+	return NSB_OK;
+}
+
+extern "C" NsbStatus nsb_mesh_download(NsbContext* c, float* vertices, float* normals, float* colors, uint64_t vertex_rows, uint32_t* indices,
+                                       uint64_t index_capacity) {
+	if (!c) return fail(NSB_ERR_INVALID, "null context");
+	if (!c->has_mesh) return fail(NSB_ERR_STATE, "nsb_mesh_download: no mesh (nsb_marching_cubes)");
+	const uint64_t rows = (c->mesh_nv + 127ull) & ~127ull;
+	if ((vertices || normals || colors) && vertex_rows > rows)
+		return fail(NSB_ERR_INVALID, "nsb_mesh_download: %llu vertex rows asked, the mesh has %llu (%llu vertices + padding)", (unsigned long long)vertex_rows,
+		            (unsigned long long)rows, (unsigned long long)c->mesh_nv);
+	if (indices && index_capacity < c->mesh_ni)
+		return fail(NSB_ERR_INVALID, "nsb_mesh_download: index buffer too small (%llu needed)", (unsigned long long)c->mesh_ni);
+	if ((normals || colors) && !c->mesh_shaded) return fail(NSB_ERR_STATE, "nsb_mesh_download: normals and colours need nsb_mesh_shade");
+	CU(cudaSetDevice(c->device));
+	CU(cudaDeviceSynchronize());
+	if (vertex_rows) {
+		if (vertices) CU(cudaMemcpy(vertices, c->mesh_verts.get(), 3 * vertex_rows * 4, cudaMemcpyDeviceToHost));
+		if (normals) CU(cudaMemcpy(normals, c->mesh_normals.get(), 3 * vertex_rows * 4, cudaMemcpyDeviceToHost));
+		if (colors) CU(cudaMemcpy(colors, c->mesh_colors.get(), 3 * vertex_rows * 4, cudaMemcpyDeviceToHost));
+	}
+	if (indices && c->mesh_ni) CU(cudaMemcpy(indices, c->mesh_idx.get(), c->mesh_ni * 4, cudaMemcpyDeviceToHost));
 	return NSB_OK;
 }

@@ -157,4 +157,20 @@ inline uint32_t render_nerf(NerfTracer& tracer, const NsbFrame& frame, float* fr
 	return tracer.trace(f, frame_buffer_dev, depth_buffer_dev, stream, synchronise);
 }
 
+// Testbed::marching_cubes (testbed_nerf.cu:4614-4649): density on the grid, marching cubes, normals and colours. The mesh stays in the
+// context; the return value is the triangle count, like the reference's. density_dev: caller scratch of res[0]*res[1]*res[2] floats
+// (res rounded up to multiples of 16 here, as the reference does); NULL meshes an existing grid given as grid_dev instead
+// (GrowingSelection::extract_fine_mesh's selection grid, growing_selection.cu:2096-2162), then without shading.
+struct Mesh { uint64_t n_vertices = 0, n_indices = 0; };
+inline Mesh marching_cubes(Context& ctx, NsbGridQuery q, float* density_dev, float thresh, int32_t rgb_activation, bool linear_colors, void* stream,
+                           const float* grid_dev = nullptr) {
+	for (int a = 0; a < 3; ++a) q.res[a] = (q.res[a] + 15) / 16 * 16;
+	Mesh m;
+	if (!grid_dev) check(nsb_density_on_grid(ctx.get(), &q, density_dev, stream), "nsb_density_on_grid");
+	check(nsb_marching_cubes(ctx.get(), grid_dev ? grid_dev : density_dev, q.res, q.aabb_min, q.aabb_max, thresh, &m.n_vertices, &m.n_indices, stream),
+	      "nsb_marching_cubes");
+	if (!grid_dev) check(nsb_mesh_shade(ctx.get(), q.train_aabb_min, q.train_aabb_max, rgb_activation, linear_colors ? 1 : 0, stream), "nsb_mesh_shade");
+	return m;
+}
+
 }  // namespace ngp_b200

@@ -5,6 +5,8 @@
   NerfRenderer.inference / density <- NerfNetwork::inference_mixed_precision / ::density
   NerfRenderer.map_rays / poisson_residuals <- EditOperator::map_rays / ::compute_poisson_full_residuals
   NerfRenderer.{add,reset}_edit_operator <- NerfTracer::{add,reset}_edit_operator (testbed.h:129-240)
+  NerfRenderer.density_on_grid / marching_cubes / mesh_shade / mesh_download <- Testbed::marching_cubes (testbed_nerf.cu:4614-4649);
+      nerfshop_b200.mesh builds the reference's Python-facing calls on them
 
 torch is used for device memory and streams only; every computation is a call into libnerfshop_b200.so.
 """
@@ -311,3 +313,47 @@ class NerfRenderer:
                                                      torch.cuda.current_stream().cuda_stream), "nsb_march_trace")
         torch.cuda.synchronize()
         return rec.cpu().numpy(), idx.cpu().numpy().view(np.uint32), cnt.cpu().numpy().view(np.uint32)
+
+    # ---- mesh extraction (Testbed::marching_cubes, testbed_nerf.cu:4614-4649) -----------------------------------------------
+    def density_on_grid(self, res3d, aabb, train_aabb, out=None, stream=None):
+        """Testbed::get_density_on_grid: float32 CUDA tensor [res_z, res_y, res_x] (x fastest) of raw densities, -10000 where the running
+        density grid is empty. res3d: positive multiples of 16."""
+        torch = _torch()
+        q = abi.NsbGridQuery()
+        q.res[:] = [int(v) for v in res3d]
+        q.aabb_min[:], q.aabb_max[:] = [float(v) for v in aabb[0]], [float(v) for v in aabb[1]]
+        q.train_aabb_min[:], q.train_aabb_max[:] = [float(v) for v in train_aabb[0]], [float(v) for v in train_aabb[1]]
+        if out is None:
+            out = torch.empty((max(q.res[2], 0), max(q.res[1], 0), max(q.res[0], 0)), dtype=torch.float32, device=torch.device("cuda", self.device))
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_density_on_grid(self.ctx, C.byref(q), out.data_ptr(), s), "nsb_density_on_grid")
+        return out
+
+    def marching_cubes(self, density, res3d, aabb, thresh: float, stream=None):
+        """marching_cubes_gpu on a float32 CUDA tensor of res3d points (x fastest): (n_vertices, n_indices) of the mesh the context now holds."""
+        torch = _torch()
+        res = (C.c_int32 * 3)(*[int(v) for v in res3d])
+        mn, mx = (C.c_float * 3)(*[float(v) for v in aabb[0]]), (C.c_float * 3)(*[float(v) for v in aabb[1]])
+        nv, ni = C.c_uint64(), C.c_uint64()
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_marching_cubes(self.ctx, density.data_ptr(), res, mn, mx, float(thresh), C.byref(nv), C.byref(ni), s), "nsb_marching_cubes")
+        return nv.value, ni.value
+
+    def mesh_shade(self, train_aabb, rgb_activation: int = abi.NSB_ACT_LOGISTIC, linear_colors: bool = False, stream=None):
+        """Vertex normals (compute_mesh_1ring) and colours (compute_mesh_vertex_colors) of the context's mesh."""
+        torch = _torch()
+        mn, mx = (C.c_float * 3)(*[float(v) for v in train_aabb[0]]), (C.c_float * 3)(*[float(v) for v in train_aabb[1]])
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_mesh_shade(self.ctx, mn, mx, int(rgb_activation), int(bool(linear_colors)), s), "nsb_mesh_shade")
+
+    def mesh_download(self, n_vertices: int, n_indices: int, padded: bool = True, shaded: bool = True) -> dict:
+        """The mesh as numpy arrays: V, N (not normalised), C with n_vertices rows (rounded up to 128 when padded, as the reference
+        allocates them), F [n_indices / 3, 3] uint32."""
+        rows = ((n_vertices + 127) // 128) * 128 if padded else n_vertices
+        V = np.zeros((rows, 3), np.float32)
+        N = np.zeros((rows, 3), np.float32) if shaded else None
+        Cc = np.zeros((rows, 3), np.float32) if shaded else None
+        F = np.zeros((n_indices // 3, 3), np.uint32)
+        abi.check(self.lib, self.lib.nsb_mesh_download(self.ctx, V.ctypes.data, None if N is None else N.ctypes.data, None if Cc is None else Cc.ctypes.data,
+                                                       rows, F.ctypes.data, F.size), "nsb_mesh_download")
+        return dict(V=V, N=N, C=Cc, F=F)

@@ -1,0 +1,188 @@
+"""Mesh extraction on the H100 (nsb_density_on_grid, nsb_marching_cubes, nsb_mesh_shade, nsb_mesh_download) on the synthetic fox-config
+scene over its render AABB [-1.5, 2.5]^3. The running density grid is the occupancy bitfield as 0/1 floats, so the filter is active
+(-10000) on empty cascade cells. Threshold: the median raw density of the unfiltered points, at which the surface is closed (every
+grid point on the box boundary is filtered)."""
+import ctypes as C
+
+import numpy as np
+import pytest
+
+import mesh_oracle as mo
+
+pytestmark = pytest.mark.gpu
+
+AABB = ((-1.5, -1.5, -1.5), (2.5, 2.5, 2.5))
+
+
+@pytest.fixture(scope="module")
+def mr(scene, built_lib):
+    import torch
+
+    if not torch.cuda.is_available():
+        pytest.skip("no CUDA device")
+    from nerfshop_b200.renderer import NerfRenderer
+
+    model, occ = scene
+    r = NerfRenderer(0)
+    r.upload_model(model.desc, model.params)
+    r.upload_density_grid(np.unpackbits(occ, bitorder="little").astype(np.float32))
+    yield r
+    r.close()
+
+
+def _positions(res):
+    """The grid positions and warped coordinates, exactly: the AABB extent 4 and res are powers of two, so every product is exact."""
+    i = np.arange(res ** 3, dtype=np.int64)
+    xyz = np.stack([i % res, (i // res) % res, i // (res * res)], 1).astype(np.float32)
+    p = xyz * (np.float32(1.0) / np.float32(res)) * np.float32(4.0) + np.float32(-1.5)
+    return p, (p - np.float32(-1.5)) / np.float32(4.0)
+
+
+def _density(mr, res):
+    return mr.density_on_grid((res, res, res), AABB, AABB).cpu().numpy().reshape(-1)
+
+
+def _mesh(mr, res, thresh, shade=True):
+    import torch
+
+    d = mr.density_on_grid((res, res, res), AABB, AABB)
+    nv, ni = mr.marching_cubes(d, (res, res, res), AABB, thresh)
+    if shade:
+        mr.mesh_shade(AABB, 0)  # rgb activation None: colours are the raw fp16 outputs
+    torch.cuda.synchronize()
+    return d.cpu().numpy(), mr.mesh_download(nv, ni, shaded=shade), nv
+
+
+def test_density_on_grid_equals_nsb_density_and_filters_empty_cells(mr, scene):
+    res = 64
+    got = _density(mr, res)
+    p, pw = _positions(res)
+    coords = np.zeros((pw.shape[0], 7), np.float32)
+    coords[:, :3] = pw
+    coords[:, 4:] = 0.5
+    raw = mr.density(coords)[0].view(np.float16).astype(np.float32)
+    # cascaded_grid_at(unwarp(warp(p)), density_grid, mip_from_pos) of the occupancy as 0/1: the unwarp is exact here
+    from nerfshop_b200 import synthetic as syn
+
+    model, occ = scene
+    grid = np.unpackbits(occ, bitorder="little")
+    q = p - np.float32(0.5)
+    m = np.abs(q).max(1)
+    mip = np.clip(np.frexp(m)[1] + 1, 0, 4)  # mip_from_pos: frexp exponent + 1
+    mip[m == 0] = 1
+    sc = np.ldexp(np.float32(1.0), 7 - mip).astype(np.float32)
+    c = np.clip(np.floor(q * sc[:, None] + np.float32(64.0)), 0, 127).astype(np.uint32)
+    cell = syn.morton3d(c[:, 0], c[:, 1], c[:, 2]).astype(np.int64) + mip.astype(np.int64) * 128 ** 3
+    empty = grid[cell] == 0
+    assert 0 < empty.sum() < empty.size
+    np.testing.assert_array_equal(got[~empty].view(np.uint32), raw[~empty].view(np.uint32))
+    assert (got[empty] == -10000.0).all()
+
+
+def _thresh(d):
+    v = d[d > -10000.0]
+    return float(np.median(v))
+
+
+def test_marching_cubes_matches_the_oracle_and_is_deterministic(mr):
+    res = 128
+    d0, m0, nv = _mesh(mr, res, 0.0, shade=False)
+    t = _thresh(d0)
+    d, m, nv = _mesh(mr, res, t)
+    V, F = mo.marching_cubes(d.reshape(res, res, res), AABB[0], AABB[1], t)
+    assert nv == V.shape[0] > 1000 and m["V"].shape[0] == ((nv + 127) // 128) * 128
+    np.testing.assert_array_equal(m["V"][:nv].view(np.uint32), V.view(np.uint32))
+    assert (m["V"][nv:] == 0).all() and (m["N"][nv:] == 0).all()
+    np.testing.assert_array_equal(m["F"], F)
+    assert mo.edge_manifold(F)
+    _, m2, _ = _mesh(mr, res, t)
+    for k in ("V", "N", "C", "F"):
+        assert m[k].tobytes() == m2[k].tobytes(), k
+
+
+def test_normals_and_colours(mr):
+    res = 64
+    d0 = _density(mr, res)
+    t = _thresh(d0)
+    d, m, nv = _mesh(mr, res, t)
+    V, N, Cc, F = m["V"], m["N"], m["C"], m["F"].astype(np.int64)
+    # normals: (pb - pa) x (pa - pc) per triangle, summed in triangle order; the device contracts the cross product into FMAs, so
+    # compare in angle
+    pa, pb, pc = V[F[:, 0]].astype(np.float64), V[F[:, 1]].astype(np.float64), V[F[:, 2]].astype(np.float64)
+    tn = np.cross(pb - pa, pa - pc)
+    ref = np.zeros((V.shape[0], 3))
+    for k in range(3):
+        np.add.at(ref, F[:, k], tn)
+    cosang = np.einsum("ij,ij->i", ref[:nv], N[:nv]) / (np.linalg.norm(ref[:nv], axis=1) * np.linalg.norm(N[:nv], axis=1))
+    assert (cosang > 1 - 1e-6).all()
+    # colours: the network at {warp(pos), warp(normalize(pos - 0.5))}; rows where the float64 direction rounds like the device's
+    dd = V.astype(np.float64) - 0.5
+    n = np.sqrt((dd * dd).sum(1))
+    dirs = np.where(n[:, None] > 0, dd / np.where(n > 0, n, 1)[:, None], dd).astype(np.float32)
+    coords = np.zeros((V.shape[0], 7), np.float32)
+    coords[:, :3] = (V - np.float32(-1.5)) / np.float32(4.0)
+    coords[:, 4:] = (dirs + np.float32(1.0)) * np.float32(0.5)
+    raw = mr.inference(coords)[:3].view(np.float16).astype(np.float32).T
+    same = (raw == Cc).all(1)
+    assert same.mean() > 0.99  # direction bits may differ in the last place where float64 rounds differently from the FMA form
+    assert np.abs(raw - Cc).max() < 2e-2
+
+
+def test_256_mesh_is_edge_manifold_and_reused_context_matches_fresh(mr, scene):
+    from nerfshop_b200.renderer import NerfRenderer
+
+    d64 = _density(mr, 64)
+    t = _thresh(d64)
+    _mesh(mr, 64, t)
+    d, m, nv = _mesh(mr, 256, t)
+    dd = d.reshape(256, 256, 256)
+    assert (dd[[0, -1]] <= t).all() and (dd[:, [0, -1]] <= t).all() and (dd[:, :, [0, -1]] <= t).all()
+    assert nv > 0 and mo.edge_manifold(m["F"])
+    model, occ = scene
+    fresh = NerfRenderer(0)
+    fresh.upload_model(model.desc, model.params)
+    fresh.upload_density_grid(np.unpackbits(occ, bitorder="little").astype(np.float32))
+    _, mf, nvf = _mesh(fresh, 256, t)
+    fresh.close()
+    assert nvf == nv
+    for k in ("V", "N", "C", "F"):
+        assert m[k].tobytes() == mf[k].tobytes(), k
+
+
+def test_status_codes(scene, built_lib):
+    import torch
+
+    if not torch.cuda.is_available():
+        pytest.skip("no CUDA device")
+    from nerfshop_b200 import abi
+    from nerfshop_b200.renderer import NerfRenderer
+
+    model, occ = scene
+    r = NerfRenderer(0)
+    out = torch.zeros(16 ** 3, device="cuda")
+    q = abi.NsbGridQuery()
+    q.res[:] = [16, 16, 16]
+    q.aabb_min[:] = q.train_aabb_min[:] = AABB[0]
+    q.aabb_max[:] = q.train_aabb_max[:] = AABB[1]
+    assert r.lib.nsb_density_on_grid(r.ctx, C.byref(q), out.data_ptr(), None) == abi.NSB_ERR_STATE  # no model
+    r.upload_model(model.desc, model.params)
+    assert r.lib.nsb_density_on_grid(r.ctx, C.byref(q), out.data_ptr(), None) == abi.NSB_ERR_STATE  # no density grid
+    r.upload_density_grid(np.unpackbits(occ, bitorder="little").astype(np.float32))
+    assert r.lib.nsb_density_on_grid(r.ctx, C.byref(q), out.data_ptr(), None) == abi.NSB_OK
+    for bad in ([17, 16, 16], [16, 0, 16], [16, 16, -16]):
+        q.res[:] = bad
+        assert r.lib.nsb_density_on_grid(r.ctx, C.byref(q), out.data_ptr(), None) == abi.NSB_ERR_INVALID
+        res = (C.c_int32 * 3)(*bad)
+        mn, mx = (C.c_float * 3)(*AABB[0]), (C.c_float * 3)(*AABB[1])
+        assert r.lib.nsb_marching_cubes(r.ctx, out.data_ptr(), res, mn, mx, 0.0, None, None, None) == abi.NSB_ERR_INVALID
+    assert r.lib.nsb_mesh_download(r.ctx, None, None, None, 0, None, 0) == abi.NSB_ERR_STATE  # no mesh yet
+    d = r.density_on_grid((64, 64, 64), AABB, AABB)
+    nv, ni = r.marching_cubes(d, (64, 64, 64), AABB, _thresh(d.cpu().numpy().reshape(-1)))
+    assert nv > 0 and ni > 0
+    V = np.zeros((nv + 128, 3), np.float32)
+    F = np.zeros(ni, np.uint32)
+    assert r.lib.nsb_mesh_download(r.ctx, None, V.ctypes.data, None, nv, None, 0) == abi.NSB_ERR_STATE  # normals before nsb_mesh_shade
+    assert r.lib.nsb_mesh_download(r.ctx, V.ctypes.data, None, None, ((nv + 127) // 128) * 128 + 1, None, 0) == abi.NSB_ERR_INVALID
+    assert r.lib.nsb_mesh_download(r.ctx, None, None, None, 0, F.ctypes.data, ni - 1) == abi.NSB_ERR_INVALID
+    assert r.lib.nsb_mesh_download(r.ctx, V.ctypes.data, None, None, nv, F.ctypes.data, ni) == abi.NSB_OK
+    r.close()
