@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define NSB_ABI_VERSION 4
+#define NSB_ABI_VERSION 5
 
 /* reference: common_nerf.h:16-39 */
 #define NSB_NERF_GRIDSIZE 128u
@@ -445,6 +445,31 @@ NsbStatus nsb_mesh_shade(NsbContext* ctx, const float train_aabb_min[3], const f
  * at the origin with a zero normal and the network's colour there. indices: [index_capacity >= n_indices]. */
 NsbStatus nsb_mesh_download(NsbContext* ctx, float* vertices, float* normals, float* colors, uint64_t vertex_rows, uint32_t* indices,
                             uint64_t index_capacity);
+
+/* ---- mesh optimisation (ABI 5): Testbed::optimise_mesh_step (testbed_nerf.cu:4470-4513), the GUI's "Optimize mesh" (testbed.cu:992-995,
+ * 1759-1761) ---------------------------------------------------------------------------------------------------------------------------- */
+/* replaces NerfNetwork::input_gradient(stream, 3, ...) together with NerfNetwork::density: the gradient of the raw density output with
+ * respect to the warped position (not rescaled to world units), through the density MLP and the hash grid, under the context's accumulator
+ * policy. coords_dev: n NerfCoordinate rows as for nsb_density. grad_dev: the 3 position floats of row i at grad_dev + i * grad_stride_floats
+ * (nothing else is written; grad_dev == coords_dev with stride 7 is allowed, as the reference calls it in place). density_fp16_dev (may be
+ * NULL): fp16 [n_padded], the raw density = row 0 of nsb_density's output. dfeat_fp16_dev (may be NULL): fp16 [32 x n_padded] row-major,
+ * dL/d(grid features) scaled by 128 (tcnn's backprop_scale). NSB_ERR_STATE without a model. Stream-ordered. */
+NsbStatus nsb_density_gradient(NsbContext* ctx, const float* coords_dev, uint32_t n, float* grad_dev, uint32_t grad_stride_floats, uint16_t* density_fp16_dev,
+                               uint16_t* dfeat_fp16_dev, uint32_t n_padded, void* stream);
+/* The members of Testbed::m_mesh that optimise_mesh_step reads (testbed.h; defaults marching_cubes.h:32-34: 2048, 128, 1). */
+typedef struct {
+	float thresh;                                 /* m_mesh.thresh: the iso-value the vertices are pushed towards */
+	float smooth_amount, density_amount, inflate_amount;
+	float train_aabb_min[3], train_aabb_max[3];   /* m_aabb */
+} NsbMeshOptimise;
+/* replaces Testbed::optimise_mesh_step(n_steps) on the context's mesh: per step, the density and its position gradient at every vertex row
+ * (the padding rows included), the 1-ring centroid and area-weighted normal of each vertex (summed in triangle order), the opt gradient
+ * normalize(grad) * sign(density - thresh) * density_amount + (v - centroid) * smooth_amount - normalize(normal) * inflate_amount, and one
+ * Adam step (tcnn, learning rate 1e-4, beta1 0.9, beta2 0.99, epsilon 1e-8; every coordinate a non-matrix parameter with its own step
+ * counter, skipped while its gradient is 0). The indices do not change and the colours are not recomputed; the normals left behind are those
+ * of the positions before the last step. Adam state (48 B per vertex row) is allocated on the first call and restarts with the first call
+ * after each nsb_marching_cubes. NSB_ERR_STATE without a model or a mesh. Stream-ordered. */
+NsbStatus nsb_mesh_optimise(NsbContext* ctx, const NsbMeshOptimise* params, uint32_t n_steps, void* stream);
 
 #ifdef __cplusplus
 }

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libnerfshop_b200.so")
 
-NSB_ABI_VERSION = 4
+NSB_ABI_VERSION = 5
 NSB_MLP_ACC_F32, NSB_MLP_ACC_F16 = 0, 1
 NSB_NERF_GRIDSIZE = 128
 NSB_NERF_CASCADES = 5
@@ -130,6 +130,12 @@ class NsbGridQuery(C.Structure):
     _fields_ = [("res", i32 * 3), ("aabb_min", f32 * 3), ("aabb_max", f32 * 3), ("train_aabb_min", f32 * 3), ("train_aabb_max", f32 * 3)]
 
 
+class NsbMeshOptimise(C.Structure):
+    """The members of Testbed::m_mesh that Testbed::optimise_mesh_step (testbed_nerf.cu:4470-4513) reads."""
+    _fields_ = [("thresh", f32), ("smooth_amount", f32), ("density_amount", f32), ("inflate_amount", f32),
+                ("train_aabb_min", f32 * 3), ("train_aabb_max", f32 * 3)]
+
+
 # every symbol include/nerfshop_b200.h declares (tests/test_abi.py checks the .so exports all of them)
 EXPORTED_SYMBOLS = [
     "nsb_abi_version", "nsb_last_error", "nsb_create", "nsb_destroy",
@@ -142,6 +148,7 @@ EXPORTED_SYMBOLS = [
     "nsb_map_positions", "nsb_poisson_residual_density", "nsb_march_trace",
     "nsb_build_tet_grid", "nsb_compute_mvc", "nsb_interpolate_with_mvc", "nsb_local_rotations",
     "nsb_density_on_grid", "nsb_marching_cubes", "nsb_mesh_shade", "nsb_mesh_download",
+    "nsb_density_gradient", "nsb_mesh_optimise",
 ]
 
 _lib = None
@@ -215,6 +222,8 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.nsb_marching_cubes.argtypes = [vp, vp, C.POINTER(i32), C.POINTER(f32), C.POINTER(f32), f32, C.POINTER(u64), C.POINTER(u64), vp]
     lib.nsb_mesh_shade.argtypes = [vp, C.POINTER(f32), C.POINTER(f32), i32, i32, vp]
     lib.nsb_mesh_download.argtypes = [vp, vp, vp, vp, u64, vp, u64]
+    lib.nsb_density_gradient.argtypes = [vp, vp, u32, vp, u32, vp, vp, u32, vp]
+    lib.nsb_mesh_optimise.argtypes = [vp, C.POINTER(NsbMeshOptimise), u32, vp]
     for name in EXPORTED_SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("nsb_last_error", "nsb_abi_version"):

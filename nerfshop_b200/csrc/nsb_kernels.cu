@@ -919,6 +919,7 @@ __global__ void k_unpack_gathered(const float4* __restrict__ gathered, const flo
 }
 
 #include "nsb_mesh.cuh"
+#include "nsb_mesh_opt.cuh"
 
 // =====================================================================================================
 // host side: context, uploads, C ABI
@@ -1024,8 +1025,16 @@ struct NsbContext {
 	bool has_mesh = false, mesh_shaded = false;
 	DevBuf<uint32_t> mc_voff, mc_tiles;  // first vertex id per grid point (4 B per point), per-tile vertex and triangle offsets
 	DevBuf<unsigned long long> mc_totals;
-	DevBuf<uint32_t> mesh_start, mesh_cursor, mesh_adj;  // per-vertex triangle lists of nsb_mesh_shade
+	DevBuf<uint32_t> mesh_start, mesh_cursor, mesh_adj;  // per-vertex triangle lists (CSR) of nsb_mesh_shade and nsb_mesh_optimise
 	DevBuf<uint8_t> mesh_scan_tmp;
+	bool mesh_csr = false;      // mesh_start / mesh_adj describe the current mesh
+	bool mesh_normals_ok = false;  // mesh_normals describe the current mesh (nsb_mesh_shade, nsb_mesh_optimise)
+	// nsb_mesh_optimise: Adam state per vertex row (moments, step counters: 36 B) and the ping-pong position buffer (12 B), allocated on the
+	// first call and reset by the first call after each nsb_marching_cubes; density (2 B) and position gradient (12 B) of the current step
+	DevBuf<float> opt_pos, opt_m1, opt_m2, opt_grad;
+	DevBuf<uint32_t> opt_steps;
+	DevBuf<__half> opt_dens;
+	bool opt_fresh = true;
 
 	~NsbContext() {  // the device arrays free themselves
 		for (cudaEvent_t e : {ev0, ev1, evm, render_done[0], render_done[1], copy_done[0], copy_done[1]}) if (e) cudaEventDestroy(e);
@@ -1143,6 +1152,9 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 		for (const void* f : {(const void*)mesh::k_density_on_grid<false>, (const void*)mesh::k_density_on_grid<true>, (const void*)mesh::k_mesh_colors<false>,
 		                      (const void*)mesh::k_mesh_colors<true>})
 			CU(set_smem(f, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
+		for (const void* f : {(const void*)meshopt::k_density_gradient<false, false>, (const void*)meshopt::k_density_gradient<true, false>,
+		                      (const void*)meshopt::k_density_gradient<false, true>, (const void*)meshopt::k_density_gradient<true, true>})
+			CU(set_smem(f, sizeof(meshopt::GradSmem), c->inference_ctas_per_sm));
 	}
 	if (getenv("NSB_VERBOSE"))
 		fprintf(stderr, "[nsb] device %d: %d SMs; k_render_fused %d tiles/CTA (%d with operators), %d regs, %zu B smem; inference %d CTAs/SM, grid update %d CTAs/SM\n", device, c->sm_count,
@@ -2100,7 +2112,8 @@ extern "C" NsbStatus nsb_marching_cubes(NsbContext* c, const float* density_dev,
 	if (!grid_res_ok(res)) return fail(NSB_ERR_INVALID, "nsb_marching_cubes: res must be positive multiples of 16 with a 32-bit point count");
 	CU(cudaSetDevice(c->device));
 	cudaStream_t st = (cudaStream_t)stream_;
-	c->has_mesh = c->mesh_shaded = false;
+	c->has_mesh = c->mesh_shaded = c->mesh_csr = c->mesh_normals_ok = false;
+	c->opt_fresh = true;  // Testbed::marching_cubes creates a fresh optimiser (testbed_nerf.cu:4638-4645)
 	c->mesh_nv = c->mesh_ni = 0;
 	mesh::McGrid g;
 	g.d = density_dev;
@@ -2139,18 +2152,11 @@ extern "C" NsbStatus nsb_marching_cubes(NsbContext* c, const float* density_dev,
 	return NSB_OK;
 }
 
-extern "C" NsbStatus nsb_mesh_shade(NsbContext* c, const float* train_aabb_min, const float* train_aabb_max, int32_t rgb_activation, int32_t linear_colors, void* stream_) {
-	if (!c || !train_aabb_min || !train_aabb_max) return fail(NSB_ERR_INVALID, "null argument");
-	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_mesh_shade: nsb_upload_model has not been called");
-	if (!c->has_mesh) return fail(NSB_ERR_STATE, "nsb_mesh_shade: no mesh (nsb_marching_cubes)");
-	if (rgb_activation < NSB_ACT_NONE || rgb_activation > NSB_ACT_EXPONENTIAL) return fail(NSB_ERR_INVALID, "nsb_mesh_shade: bad rgb_activation");
-	CU(cudaSetDevice(c->device));
-	cudaStream_t st = (cudaStream_t)stream_;
-	const uint32_t nv = (uint32_t)c->mesh_nv, rows = (uint32_t)((c->mesh_nv + 127ull) & ~127ull), nt = (uint32_t)(c->mesh_ni / 3);
-	c->mesh_shaded = false;
-	if (rows == 0) { c->mesh_shaded = true; return NSB_OK; }
-	CU(c->mesh_normals.reserve(3 * (size_t)rows));
-	CU(c->mesh_colors.reserve(3 * (size_t)rows));
+// The per-vertex triangle lists of the current mesh, built once per mesh: degrees, their exclusive scan, then the triangle ids per vertex
+// (in slot order; the kernels that read a list visit it sorted)
+static NsbStatus mesh_build_csr(NsbContext* c, cudaStream_t st) {
+	if (c->mesh_csr) return NSB_OK;
+	const uint32_t nv = (uint32_t)c->mesh_nv, nt = (uint32_t)(c->mesh_ni / 3);
 	CU(c->mesh_start.reserve((size_t)nv + 1));
 	CU(c->mesh_cursor.reserve((size_t)nv + 1));
 	CU(c->mesh_adj.reserve(nt ? (size_t)3 * nt : 1));
@@ -2162,6 +2168,25 @@ extern "C" NsbStatus nsb_mesh_shade(NsbContext* c, const float* train_aabb_min, 
 	CU(cub::DeviceScan::ExclusiveSum(c->mesh_scan_tmp.get(), tmp_bytes, c->mesh_cursor.get(), c->mesh_start.get(), nv + 1, st));
 	CU(cudaMemsetAsync(c->mesh_cursor.get(), 0, ((size_t)nv + 1) * 4, st));
 	if (nt) mesh::k_mesh_fill<<<(nt + 255) / 256, 256, 0, st>>>(nt, c->mesh_idx.get(), c->mesh_start.get(), c->mesh_cursor.get(), c->mesh_adj.get());
+	CU(cudaGetLastError());
+	c->mesh_csr = true;
+	return NSB_OK;
+}
+
+extern "C" NsbStatus nsb_mesh_shade(NsbContext* c, const float* train_aabb_min, const float* train_aabb_max, int32_t rgb_activation, int32_t linear_colors, void* stream_) {
+	if (!c || !train_aabb_min || !train_aabb_max) return fail(NSB_ERR_INVALID, "null argument");
+	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_mesh_shade: nsb_upload_model has not been called");
+	if (!c->has_mesh) return fail(NSB_ERR_STATE, "nsb_mesh_shade: no mesh (nsb_marching_cubes)");
+	if (rgb_activation < NSB_ACT_NONE || rgb_activation > NSB_ACT_EXPONENTIAL) return fail(NSB_ERR_INVALID, "nsb_mesh_shade: bad rgb_activation");
+	CU(cudaSetDevice(c->device));
+	cudaStream_t st = (cudaStream_t)stream_;
+	const uint32_t nv = (uint32_t)c->mesh_nv, rows = (uint32_t)((c->mesh_nv + 127ull) & ~127ull);
+	c->mesh_shaded = false;
+	if (rows == 0) { c->mesh_shaded = c->mesh_normals_ok = true; return NSB_OK; }
+	CU(c->mesh_normals.reserve(3 * (size_t)rows));
+	CU(c->mesh_colors.reserve(3 * (size_t)rows));
+	const NsbStatus csr = mesh_build_csr(c, st);
+	if (csr != NSB_OK) return csr;
 	mesh::k_mesh_normals<<<(rows + 255) / 256, 256, 0, st>>>(nv, rows, c->mesh_verts.get(), c->mesh_idx.get(), c->mesh_start.get(), c->mesh_adj.get(),
 	                                                        c->mesh_normals.get());
 	mesh::Aabb train;
@@ -2172,7 +2197,7 @@ extern "C" NsbStatus nsb_mesh_shade(NsbContext* c, const float* train_aabb_min, 
 	(c->acc16 ? mesh::k_mesh_colors<true> : mesh::k_mesh_colors<false>)<<<grid, 128, sizeof(tc::TileSmem), st>>>(
 		c->model, rows, c->mesh_verts.get(), train, rgb_activation, linear_colors ? 1 : 0, c->mesh_colors.get());
 	CU(cudaGetLastError());
-	c->mesh_shaded = true;
+	c->mesh_shaded = c->mesh_normals_ok = true;
 	return NSB_OK;
 }
 
@@ -2186,7 +2211,8 @@ extern "C" NsbStatus nsb_mesh_download(NsbContext* c, float* vertices, float* no
 		            (unsigned long long)rows, (unsigned long long)c->mesh_nv);
 	if (indices && index_capacity < c->mesh_ni)
 		return fail(NSB_ERR_INVALID, "nsb_mesh_download: index buffer too small (%llu needed)", (unsigned long long)c->mesh_ni);
-	if ((normals || colors) && !c->mesh_shaded) return fail(NSB_ERR_STATE, "nsb_mesh_download: normals and colours need nsb_mesh_shade");
+	if ((normals && !c->mesh_normals_ok) || (colors && !c->mesh_shaded))
+		return fail(NSB_ERR_STATE, "nsb_mesh_download: normals need nsb_mesh_shade or nsb_mesh_optimise, colours nsb_mesh_shade");
 	CU(cudaSetDevice(c->device));
 	CU(cudaDeviceSynchronize());
 	if (vertex_rows) {
@@ -2195,5 +2221,77 @@ extern "C" NsbStatus nsb_mesh_download(NsbContext* c, float* vertices, float* no
 		if (colors) CU(cudaMemcpy(colors, c->mesh_colors.get(), 3 * vertex_rows * 4, cudaMemcpyDeviceToHost));
 	}
 	if (indices && c->mesh_ni) CU(cudaMemcpy(indices, c->mesh_idx.get(), c->mesh_ni * 4, cudaMemcpyDeviceToHost));
+	return NSB_OK;
+}
+
+// ---- mesh optimisation (Testbed::optimise_mesh_step, testbed_nerf.cu:4470-4513) ---------------------------------------------
+extern "C" NsbStatus nsb_density_gradient(NsbContext* c, const float* coords, uint32_t n, float* grad, uint32_t grad_stride_floats, uint16_t* density_fp16,
+                                          uint16_t* dfeat_fp16, uint32_t n_padded, void* stream) {
+	if (!c) return fail(NSB_ERR_INVALID, "null context");
+	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_density_gradient: nsb_upload_model has not been called");
+	if (n && (!coords || !grad)) return fail(NSB_ERR_INVALID, "nsb_density_gradient: null argument");
+	if (grad_stride_floats < 3) return fail(NSB_ERR_INVALID, "nsb_density_gradient: grad_stride_floats < 3");
+	if (n_padded < n) return fail(NSB_ERR_INVALID, "nsb_density_gradient: n_padded < n");
+	if (n_padded == 0) return NSB_OK;
+	CU(cudaSetDevice(c->device));
+	meshopt::GradIo io{};
+	io.in = coords; io.n = n; io.n_padded = n_padded;
+	io.grad = grad; io.grad_stride = grad_stride_floats;
+	io.dens = reinterpret_cast<__half*>(density_fp16); io.dfeat = reinterpret_cast<__half*>(dfeat_fp16);
+	uint32_t grid = (n_padded + 127) / 128;
+	const uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
+	if (grid > cap) grid = cap;
+	(c->acc16 ? meshopt::k_density_gradient<true, false> : meshopt::k_density_gradient<false, false>)<<<grid, 128, sizeof(meshopt::GradSmem), (cudaStream_t)stream>>>(
+		c->model, io);
+	CU(cudaGetLastError());
+	return NSB_OK;
+}
+
+extern "C" NsbStatus nsb_mesh_optimise(NsbContext* c, const NsbMeshOptimise* p, uint32_t n_steps, void* stream_) {
+	if (!c || !p) return fail(NSB_ERR_INVALID, "null argument");
+	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_mesh_optimise: nsb_upload_model has not been called");
+	if (!c->has_mesh) return fail(NSB_ERR_STATE, "nsb_mesh_optimise: no mesh (nsb_marching_cubes)");
+	const uint32_t nv = (uint32_t)c->mesh_nv, rows = (uint32_t)((c->mesh_nv + 127ull) & ~127ull);
+	if (rows == 0 || n_steps == 0) return NSB_OK;
+	CU(cudaSetDevice(c->device));
+	cudaStream_t st = (cudaStream_t)stream_;
+	const NsbStatus csr = mesh_build_csr(c, st);
+	if (csr != NSB_OK) return csr;
+	const size_t n3 = 3 * (size_t)rows;
+	CU(c->mesh_normals.reserve(n3));
+	if (c->opt_fresh || c->opt_m1.capacity() < n3) {
+		CU(c->opt_pos.reserve(n3));
+		CU(c->opt_m1.reserve(n3));
+		CU(c->opt_m2.reserve(n3));
+		CU(c->opt_steps.reserve(n3));
+		CU(c->opt_grad.reserve(n3));
+		CU(c->opt_dens.reserve(rows));
+		CU(cudaMemsetAsync(c->opt_m1.get(), 0, n3 * sizeof(float), st));
+		CU(cudaMemsetAsync(c->opt_m2.get(), 0, n3 * sizeof(float), st));
+		CU(cudaMemsetAsync(c->opt_steps.get(), 0, n3 * sizeof(uint32_t), st));
+		c->opt_fresh = false;
+	}
+	meshopt::GradIo io{};
+	io.n = rows; io.n_padded = rows;
+	io.grad_stride = 3;
+	io.dens = c->opt_dens.get();
+	io.dfeat = nullptr;
+	for (int a = 0; a < 3; ++a) { io.train.mn[a] = p->train_aabb_min[a]; io.train.mx[a] = p->train_aabb_max[a]; }
+	const meshopt::OptParams op{p->thresh, p->smooth_amount, p->density_amount, p->inflate_amount};
+	uint32_t grid = rows / 128;
+	const uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
+	if (grid > cap) grid = cap;
+	auto grad_kernel = c->acc16 ? meshopt::k_density_gradient<true, true> : meshopt::k_density_gradient<false, true>;
+	for (uint32_t s = 0; s < n_steps; ++s) {
+		io.in = c->mesh_verts.get();
+		io.grad = c->opt_grad.get();
+		grad_kernel<<<grid, 128, sizeof(meshopt::GradSmem), st>>>(c->model, io);
+		meshopt::k_mesh_opt_step<<<(rows + 255) / 256, 256, 0, st>>>(nv, rows, c->mesh_verts.get(), c->opt_pos.get(), c->mesh_idx.get(), c->mesh_start.get(),
+		                                                            c->mesh_adj.get(), c->opt_dens.get(), c->opt_grad.get(), op, c->opt_m1.get(), c->opt_m2.get(),
+		                                                            c->opt_steps.get(), c->mesh_normals.get());
+		CU(cudaGetLastError());
+		std::swap(c->mesh_verts, c->opt_pos);  // the new positions become the mesh; the old buffer is the next step's output
+	}
+	c->mesh_normals_ok = true;
 	return NSB_OK;
 }

@@ -160,6 +160,23 @@ template <> __device__ __forceinline__ void wgmma_rs<64, true>(uint32_t* d, cons
 		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
 		: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
 }
+// N = 32: the backward of the density MLP's first layer (nsb_mesh_opt.cuh), D = dL/dh * W1 against a W1^T operand
+template <> __device__ __forceinline__ void wgmma_rs<32, false>(uint32_t* d, const uint32_t* a, uint64_t bd, uint32_t scale_d) {
+	asm volatile(
+		"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+		: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_rs<32, true>(uint32_t* d, const uint32_t* a, uint64_t bd, uint32_t scale_d) {
+	asm volatile(
+		"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n32k16.f16.f16.f16 "
+		"{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+		: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
+}
 template <> __device__ __forceinline__ void wgmma_rs<16, false>(uint32_t* d, const uint32_t* a, uint64_t bd, uint32_t scale_d) {
 	asm volatile(
 		"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"

@@ -2,7 +2,7 @@
 // member signatures for the render path, so that Testbed::render_frame (src/testbed.cu:2632-2648) can call it the way
 // it calls the stock code. Header-only; Eigen-free (cameras are passed as 12 floats, column-major like Eigen's storage).
 //
-//   ngp_b200::NerfNetwork      <- NerfNetwork<T>            (nerf_network.h:87-120): inference_mixed_precision, density
+//   ngp_b200::NerfNetwork      <- NerfNetwork<T>            (nerf_network.h:87-120): inference_mixed_precision, density, input_gradient(3)
 //   ngp_b200::EditOperator     <- EditOperator              (editing/edit_operator.h:25-94): the POD handed to the tracer + the four device
 //                                                            virtuals (map_rays, map_positions, compute_poisson_full_residuals,
 //                                                            compute_poisson_residual_density) once the operator is attached to a tracer
@@ -58,6 +58,12 @@ public:
 	}
 	void density(void* stream, const float* input_dev, uint16_t* output_dev, uint32_t n, uint32_t n_padded) const {
 		check(nsb_density(m_ctx->get(), input_dev, n, output_dev, n_padded, stream), "nsb_density");
+	}
+	// NerfNetwork::input_gradient (nerf_network_full.h:142-221) for the density output (dim 3) only: the gradient w.r.t. the warped
+	// position into the first 3 floats of each output row (output_dev == input_dev is allowed, as the reference calls it in place)
+	void input_gradient(void* stream, uint32_t dim, const float* input_dev, float* output_dev, uint32_t output_stride_floats, uint32_t n, uint32_t n_padded) const {
+		if (dim != 3) throw std::runtime_error("NerfNetwork::input_gradient: only dim 3 (the density) is implemented");
+		check(nsb_density_gradient(m_ctx->get(), input_dev, n, output_dev, output_stride_floats, nullptr, nullptr, n_padded, stream), "nsb_density_gradient");
 	}
 
 private:
@@ -171,6 +177,11 @@ inline Mesh marching_cubes(Context& ctx, NsbGridQuery q, float* density_dev, flo
 	      "nsb_marching_cubes");
 	if (!grid_dev) check(nsb_mesh_shade(ctx.get(), q.train_aabb_min, q.train_aabb_max, rgb_activation, linear_colors ? 1 : 0, stream), "nsb_mesh_shade");
 	return m;
+}
+
+// Testbed::optimise_mesh_step (testbed_nerf.cu:4470-4513) on the context's mesh, with m_mesh's thresh and amounts in `p`.
+inline void optimise_mesh_step(Context& ctx, const NsbMeshOptimise& p, uint32_t n_steps, void* stream) {
+	check(nsb_mesh_optimise(ctx.get(), &p, n_steps, stream), "nsb_mesh_optimise");
 }
 
 }  // namespace ngp_b200

@@ -5,6 +5,7 @@ nsb_mesh_shade, nsb_mesh_download).
   compute_marching_cubes_mesh   <- Testbed::compute_marching_cubes_mesh (python_api.cu:105-126) over Testbed::marching_cubes
   save_mesh                     <- save_mesh (marching_cubes.cu:760-896)
   compute_and_save_marching_cubes_mesh <- Testbed::compute_and_save_marching_cubes_mesh (testbed.cu:337-343)
+  optimise_mesh_step            <- Testbed::optimise_mesh_step (testbed_nerf.cu:4470-4513), the GUI's "Optimize mesh"
 
 Arrays have the reference's row count: n_vertices rounded up to 128 (marching_cubes.cu:751-753). The padding rows sit at the
 origin, carry the network's colour there and a zero normal.
@@ -95,3 +96,11 @@ def compute_and_save_marching_cubes_mesh(renderer, path: str, res3d, aabb, thres
     nv, ni = renderer.marching_cubes(density, res, aabb, thresh)
     renderer.mesh_shade(train_aabb, rgb_activation, linear_colors)
     save_mesh(path, renderer.mesh_download(nv, ni), nerf_scale, nerf_offset)
+
+
+def optimise_mesh_step(renderer, n_steps: int, thresh: float, train_aabb, smooth_amount: float = 2048.0, density_amount: float = 128.0,
+                       inflate_amount: float = 1.0) -> None:
+    """Moves the renderer's current mesh (the last marching_cubes) towards the `thresh` iso-surface of the raw density while smoothing it:
+    n_steps Adam steps on every vertex row, padding rows included. The defaults are the reference's (marching_cubes.h:32-34). Read the result
+    with renderer.mesh_download: the normals are those of the positions before the last step; the colours are not recomputed."""
+    renderer.mesh_optimise(n_steps, thresh, train_aabb, smooth_amount, density_amount, inflate_amount)

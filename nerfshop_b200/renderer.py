@@ -346,6 +346,34 @@ class NerfRenderer:
         s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
         abi.check(self.lib, self.lib.nsb_mesh_shade(self.ctx, mn, mx, int(rgb_activation), int(bool(linear_colors)), s), "nsb_mesh_shade")
 
+    # ---- mesh optimisation (Testbed::optimise_mesh_step, testbed_nerf.cu:4470-4513) ---------------------------------------------
+    def density_gradient(self, coords, want_dfeat: bool = False):
+        """NerfNetwork::density + input_gradient(3) on NerfCoordinate rows: (grad float32 [n, 3] w.r.t. the warped position, raw density
+        fp16 bits uint16 [n][, dL/dfeatures * 128 as fp16 bits uint16 [32, n]])."""
+        torch = _torch()
+        c = self._coords(coords)
+        n = c.shape[0]
+        n_pad = ((n + 127) // 128) * 128
+        grad = torch.zeros((n, 3), dtype=torch.float32, device=c.device)
+        dens = torch.zeros(n_pad, dtype=torch.int16, device=c.device)
+        dfeat = torch.zeros((32, n_pad), dtype=torch.int16, device=c.device) if want_dfeat else None
+        abi.check(self.lib, self.lib.nsb_density_gradient(self.ctx, c.data_ptr() if n else None, n, grad.data_ptr() if n else None, 3,
+                                                          dens.data_ptr() if n else None, dfeat.data_ptr() if (want_dfeat and n) else None, n_pad,
+                                                          torch.cuda.current_stream().cuda_stream), "nsb_density_gradient")
+        torch.cuda.synchronize()
+        out = (grad.cpu().numpy(), dens.cpu().numpy().view(np.uint16)[:n])
+        return out + (dfeat.cpu().numpy().view(np.uint16)[:, :n],) if want_dfeat else out
+
+    def mesh_optimise(self, n_steps: int, thresh: float, train_aabb, smooth_amount: float = 2048.0, density_amount: float = 128.0,
+                      inflate_amount: float = 1.0, stream=None):
+        """n_steps of Testbed::optimise_mesh_step on the context's mesh (its vertex rows move in place; read them with mesh_download)."""
+        torch = _torch()
+        p = abi.NsbMeshOptimise()
+        p.thresh, p.smooth_amount, p.density_amount, p.inflate_amount = float(thresh), float(smooth_amount), float(density_amount), float(inflate_amount)
+        p.train_aabb_min[:], p.train_aabb_max[:] = [float(v) for v in train_aabb[0]], [float(v) for v in train_aabb[1]]
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_mesh_optimise(self.ctx, C.byref(p), int(n_steps), s), "nsb_mesh_optimise")
+
     def mesh_download(self, n_vertices: int, n_indices: int, padded: bool = True, shaded: bool = True) -> dict:
         """The mesh as numpy arrays: V, N (not normalised), C with n_vertices rows (rounded up to 128 when padded, as the reference
         allocates them), F [n_indices / 3, 3] uint32."""
