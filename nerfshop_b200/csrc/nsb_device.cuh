@@ -11,6 +11,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cmath>
+
+#include "../../include/nerfshop_b200.h"
+
 namespace nsb {
 
 // ------------------------------------------------------------------------------------------------
@@ -571,10 +575,15 @@ __device__ __forceinline__ MarchResult next_occupied_budget(const DevFrame& f, c
 // tiny-cuda-nn GridEncoding (HashGrid, F = 2, linear) — SURVEY.md Appendix B.
 // One level: 8 gathers of a __half2, result += (half)(weight * data) with fp16 accumulation.
 // ------------------------------------------------------------------------------------------------
-// tcnn grid_index: dense levels index x + y*res + z*res^2, the others hash the vertex (primes 1, 2654435761, 805459861).
+// tcnn grid_index: dense levels index x + y*res + z*res^2, the others hash the vertex (primes 1, 2654435761, 805459861); then `% size`,
+// on the uint32 index, for every grid coordinate (positions outside [0,1]^3 wrap the coordinates through uint32).
 // MODE 0: dense, 1: hashed, 2: either (level kind is uniform across the launch: a select, not a divergent branch).
-template <int MODE>
-__device__ __forceinline__ uint32_t grid_index(const DevLevel& L, uint32_t gx, uint32_t gy, uint32_t gz) {
+// IN_RANGE: the caller guarantees every coordinate is at most res (a warped position in [-0.5/scale, 1 + 0.5/scale] and a model whose
+// dense levels satisfy dense_in_range), so a dense index is below res + res^2 + res^3 < 2*size and one conditional subtraction is the
+// modulo. Only the fused renderer's frames without operators whose render AABB lies inside the train AABB take it (render_in_range).
+__host__ __device__ __noinline__ inline uint32_t grid_mod_slow(uint32_t d, uint32_t size) { return d % size; }
+template <int MODE, bool IN_RANGE = false>
+__host__ __device__ __forceinline__ uint32_t grid_index(const DevLevel& L, uint32_t gx, uint32_t gy, uint32_t gz) {
 	uint32_t h = 0, d = 0;
 	if (MODE != 0) {
 		h = gx ^ (gy * 2654435761u) ^ (gz * 805459861u);
@@ -582,15 +591,17 @@ __device__ __forceinline__ uint32_t grid_index(const DevLevel& L, uint32_t gx, u
 	}
 	if (MODE != 1) {
 		d = gx + gy * L.res + gz * L.res2;
-		// `index % size`: a dense index is below res + res^2 + res^3 < 2*size, so one conditional subtraction is the modulo
-		d = d >= L.size ? d - L.size : d;
+		// `index % size` (dense size <= 2^24, so 2*size does not wrap). The division sits behind a branch in a call that is not inlined,
+		// so it is never if-converted into the gather loop: in-cube samples pay a compare and a branch.
+		if (IN_RANGE) d = d >= L.size ? d - L.size : d;
+		else d = d < L.size ? d : (d < 2u * L.size ? d - L.size : grid_mod_slow(d, L.size));
 	}
 	return MODE == 0 ? d : (MODE == 1 ? h : (L.hashed ? h : d));
 }
 
 // NL consecutive levels at once: all 8*NL gathers are issued before the first one is consumed (memory-level parallelism;
 // the walk is bound by L1/L2 gather throughput, not by arithmetic).
-template <int NL, int MODE>
+template <int NL, int MODE, bool IN_RANGE = false>
 __device__ __forceinline__ void encode_levels(const DevLevel* __restrict__ L, const __half2* __restrict__ grid, float x, float y, float z, __half2* out) {
 	__half2 v[NL][8];
 	float wx[NL], wy[NL], wz[NL];
@@ -599,10 +610,11 @@ __device__ __forceinline__ void encode_levels(const DevLevel* __restrict__ L, co
 		float px = fma_(L[l].scale, x, 0.5f), py = fma_(L[l].scale, y, 0.5f), pz = fma_(L[l].scale, z, 0.5f);
 		float fx = floorf(px), fy = floorf(py), fz = floorf(pz);
 		wx[l] = sub(px, fx); wy[l] = sub(py, fy); wz[l] = sub(pz, fz);
+		// (int) is cvt.rzi.s32.f32, as in tcnn: truncation, NaN -> 0, saturation outside the int range (the oracle's cvt_rzi_s32)
 		uint32_t gx = (uint32_t)(int)fx, gy = (uint32_t)(int)fy, gz = (uint32_t)(int)fz;
 		const __half2* base = L[l].base;
 #pragma unroll
-		for (int c = 0; c < 8; ++c) v[l][c] = __ldg(base + grid_index<MODE>(L[l], gx + (c & 1), gy + ((c >> 1) & 1), gz + ((c >> 2) & 1)));
+		for (int c = 0; c < 8; ++c) v[l][c] = __ldg(base + grid_index<MODE, IN_RANGE>(L[l], gx + (c & 1), gy + ((c >> 1) & 1), gz + ((c >> 2) & 1)));
 	}
 #pragma unroll
 	for (int l = 0; l < NL; ++l) {
@@ -814,6 +826,55 @@ __device__ __forceinline__ void membrane_rgb(const DevOp* __restrict__ ops, cons
 		for (int k = 1; k < 9; ++k) acc = fma_(p[k], membrane_sh(ops, m, c * 9 + k), acc);
 		rgb[c] = acc;
 	}
+}
+
+// ------------------------------------------------------------------------------------------------
+// Level table of the hash grid (host). Shared with the host build of grid_index that the CPU tests compile.
+// ------------------------------------------------------------------------------------------------
+// Accepted: the configs/nerf/base.json topology, log2_hashmap_size 1..24, base_resolution >= 1, per_level_scale >= 1 (not NaN) and every
+// level's scale below 2^32, so that tcnn's `(uint32_t)ceilf(scale) + 1` resolution is defined and fits a uint32.
+inline bool build_levels(const NsbModelDesc* d, DevLevel* L, uint64_t* n_grid_entries) {
+	if (!d || d->n_levels != 16 || d->n_features_per_level != 2 || d->n_neurons != 64 || d->n_hidden_density != 1 || d->n_hidden_rgb != 2 ||
+	    d->sh_degree != 4 || d->log2_hashmap_size == 0 || d->log2_hashmap_size > 24 || d->base_resolution == 0 || !(d->per_level_scale >= 1.0f))
+		return false;
+	float l2s = log2f(d->per_level_scale);
+	uint64_t offset = 0;
+	for (uint32_t l = 0; l < d->n_levels; ++l) {
+		float scale = exp2f((float)l * l2s) * (float)d->base_resolution - 1.0f;  // tcnn grid_scale
+		if (!(scale < 4294967296.0f)) return false;                                // also rejects inf
+		uint32_t res = (uint32_t)ceilf(scale) + 1u;                                // tcnn grid_resolution
+		double dense = (double)res * res * res;
+		uint32_t max_params = 0xffffffffu / 2;
+		uint32_t n = dense > (double)max_params ? max_params : (uint32_t)dense;
+		n = ((n + 7u) / 8u) * 8u;
+		n = n < (1u << d->log2_hashmap_size) ? n : (1u << d->log2_hashmap_size);
+		// tcnn's grid_index decides hash vs. dense with a uint32 stride: `for (dim < 3 && stride <= size) stride *= res`, hashed iff
+		// size < stride. The stride can wrap (res = 2^18 at aabb_scale 128: res^2 = 2^36 = 0 mod 2^32), and then tcnn indexes the level densely.
+		uint32_t stride = 1;
+		for (int dim = 0; dim < 3 && stride <= n; ++dim) stride *= res;
+		L[l].scale = scale;
+		L[l].res = res;
+		L[l].base = reinterpret_cast<const __half2*>((uintptr_t)offset * sizeof(__half2));  // entry offset; rebased onto the table by nsb_upload_model
+		L[l].size = n;
+		L[l].hashed = n < stride ? 1u : 0u;
+		L[l].res2 = L[l].hashed ? 0u : res * res;  // tcnn's third stride, uint32
+		// Hashed implies size = 2^log2_hashmap_size: size < stride <= res^3 with no wrap means the cap was taken; a wrap means res^3 > 2^32
+		// and the cap as well. So mask = size - 1, and grid_index takes a hashed level's `index % size` as `index & mask`.
+		L[l].mask = L[l].hashed ? n - 1 : 0u;
+		offset += n;
+	}
+	*n_grid_entries = offset;
+	return true;
+}
+
+// grid_index<MODE, true>'s condition for in-cube positions (coordinates at most res): every dense level's index stays below 2*size.
+inline bool dense_in_range(const DevLevel* L, uint32_t n_levels) {
+	for (uint32_t l = 0; l < n_levels; ++l) {
+		if (L[l].hashed) continue;
+		const uint64_t r = L[l].res;
+		if (r * r * r >= (1ull << 32) || r + r * r + r * r * r >= 2ull * L[l].size) return false;
+	}
+	return true;
 }
 
 }  // namespace nsb

@@ -129,6 +129,8 @@ __global__ void __launch_bounds__(256) k_prepare_rays(const DevFrame f, const ui
 #ifndef NSB_ENC_NL
 #define NSB_ENC_NL 2  // levels per loop iteration (8*NL gathers in flight per thread)
 #endif
+// IN_RANGE: grid_index's shortcut (nsb_device.cuh); only k_render_fused passes true, for frames where render_in_range holds.
+template <bool IN_RANGE = false>
 __device__ __forceinline__ void encode_to_a32(uint8_t* a32, const DevModel& m, bool valid, V3 pw, uint32_t row) {
 	constexpr int NL = NSB_ENC_NL;
 #pragma unroll 1
@@ -139,9 +141,9 @@ __device__ __forceinline__ void encode_to_a32(uint8_t* a32, const DevModel& m, b
 		if (valid) {
 			uint32_t mode = m.pair_mode[(NL * g) / 2];  // uniform
 			if (NL == 4 && m.pair_mode[(NL * g) / 2 + 1] != mode) mode = 2;
-			if (mode == 1) encode_levels<NL, 1>(m.levels + NL * g, m.grid, pw.x, pw.y, pw.z, h);
-			else if (mode == 0) encode_levels<NL, 0>(m.levels + NL * g, m.grid, pw.x, pw.y, pw.z, h);
-			else encode_levels<NL, 2>(m.levels + NL * g, m.grid, pw.x, pw.y, pw.z, h);
+			if (mode == 1) encode_levels<NL, 1, IN_RANGE>(m.levels + NL * g, m.grid, pw.x, pw.y, pw.z, h);
+			else if (mode == 0) encode_levels<NL, 0, IN_RANGE>(m.levels + NL * g, m.grid, pw.x, pw.y, pw.z, h);
+			else encode_levels<NL, 2, IN_RANGE>(m.levels + NL * g, m.grid, pw.x, pw.y, pw.z, h);
 		}
 		// levels NL*g .. NL*g+NL-1 = fp16 features 2*NL*g ..: NL*4 bytes of this row's k-chunk (NL*g)/4
 		uint8_t* dst = a32 + ((NL * g) >> 2) * (tc::ROWS * 16) + tc::phys_row(row) * 16 + ((NL * g) & 3) * 4;
@@ -188,7 +190,8 @@ static_assert(RENDER_TILES >= 1 && RENDER_TILES <= 8 && RENDER_TILES_OPS >= 1 &&
 // OPS = false: the instantiation for frames without edit operators (f.apply_ops == 0 or no operator uploaded) carries none of the deform /
 // membrane code in its hot loop (the loop has to fit the instruction cache).
 // ACC16: the MLP accumulator policy (nsb_set_mlp_accumulator): fp16 wgmma accumulators, like the reference's wmma __half fragments.
-template <bool OPS, bool ACC16>
+// IN_RANGE (only with OPS = false): the hash grid takes grid_index's one-subtraction modulo; the host picks it where render_in_range holds.
+template <bool OPS, bool ACC16, bool IN_RANGE>
 __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(const DevFrame f, const DevModel m, const uint8_t* __restrict__ bitfield,
                                                       const DevOp* __restrict__ ops, const int n_ops, const int any_poisson,
                                                       float4* __restrict__ fb, float* __restrict__ depth_out, const RayRec* __restrict__ list,
@@ -215,6 +218,7 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 	C.bar_id = 1 + tile;
 
 	constexpr bool ops_on = OPS;  // the host picks the instantiation: f.apply_ops && n_ops > 0
+	static_assert(!(OPS && IN_RANGE), "operators map samples anywhere: their frames take the exact grid index");
 
 	// what stays in registers across a round
 	bool alive = false, exhausted = false;  // exhausted is warp-uniform: the queue had nothing left when this warp last asked
@@ -358,7 +362,7 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 #ifdef NSB_PROFILE
 			const long long e0 = clock64();
 #endif
-			encode_to_a32(TB.a32, m, old_pass ? need_old : has_sample, old_pass ? pw_old : pw, tid);
+			encode_to_a32<IN_RANGE>(TB.a32, m, old_pass ? need_old : has_sample, old_pass ? pw_old : pw, tid);
 #ifdef NSB_PROFILE
 			enc_cycles += clock64() - e0;
 #endif
@@ -974,6 +978,7 @@ struct NsbContext {
 	bool has_model = false, has_occ = false;
 	NsbModelDesc desc{};
 	DevModel model{};
+	bool dense_in_range = false;       // the model's dense levels admit grid_index's in-range shortcut (nsb_device.cuh)
 	DevBuf<__half2> d_grid;
 	DevBuf<uint8_t> d_wimage;
 	DevBuf<__half> d_wrow;
@@ -1044,34 +1049,6 @@ struct NsbContext {
 
 static uint32_t next_multiple_u32(uint32_t v, uint32_t m) { return ((v + m - 1) / m) * m; }
 
-static bool build_levels(const NsbModelDesc* d, DevLevel* L, uint64_t* n_grid_entries) {
-	if (!d || d->n_levels != 16 || d->n_features_per_level != 2 || d->n_neurons != 64 || d->n_hidden_density != 1 || d->n_hidden_rgb != 2 ||
-	    d->sh_degree != 4 || d->log2_hashmap_size == 0 || d->log2_hashmap_size > 24 || d->base_resolution == 0 || !(d->per_level_scale > 0.0f))
-		return false;
-	float l2s = log2f(d->per_level_scale);
-	uint64_t offset = 0;
-	for (uint32_t l = 0; l < d->n_levels; ++l) {
-		float scale = exp2f((float)l * l2s) * (float)d->base_resolution - 1.0f;  // tcnn grid_scale
-		uint32_t res = (uint32_t)ceilf(scale) + 1u;                                // tcnn grid_resolution
-		double dense = (double)res * res * res;
-		uint32_t max_params = 0xffffffffu / 2;
-		uint32_t n = dense > (double)max_params ? max_params : (uint32_t)dense;
-		n = next_multiple_u32(n, 8u);
-		n = n < (1u << d->log2_hashmap_size) ? n : (1u << d->log2_hashmap_size);
-		L[l].scale = scale;
-		L[l].res = res;
-		L[l].base = reinterpret_cast<const __half2*>((uintptr_t)offset * sizeof(__half2));  // entry offset; rebased onto the table by nsb_upload_model
-		L[l].size = n;
-		L[l].hashed = dense > (double)n ? 1u : 0u;
-		L[l].res2 = L[l].hashed ? 0u : res * res;
-		// Hashed implies size = 2^log2_hashmap_size: n is res^3 rounded up to a multiple of 8 (>= res^3: dense) or the table cap.
-		// So mask = size - 1, and grid_index takes a hashed level's `index % size` as `index & mask`.
-		L[l].mask = L[l].hashed ? n - 1 : 0u;
-		offset += n;
-	}
-	*n_grid_entries = offset;
-	return true;
-}
 static const uint64_t kMlpParams = 64 * 32 + 16 * 64 + 64 * 32 + 64 * 64 + 16 * 64;
 
 extern "C" int nsb_abi_version(void) { return NSB_ABI_VERSION; }
@@ -1124,12 +1101,14 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 	};
 	// k_render_fused: ONE CTA of RENDER_TILES (RENDER_TILES_OPS with operators) tiles per SM (768 x 80 / 640 x 96 registers = the register file;
 	// shared memory 20 KB weights + 22.5 KB per tile).
-	CU(set_smem((const void*)k_render_fused<false, false>, sizeof(RenderSmemT<render_tiles(false)>), 1));
-	CU(set_smem((const void*)k_render_fused<true, false>, sizeof(RenderSmemT<render_tiles(true)>), 1));
-	CU(set_smem((const void*)k_render_fused<false, true>, sizeof(RenderSmemT<render_tiles(false)>), 1));
-	CU(set_smem((const void*)k_render_fused<true, true>, sizeof(RenderSmemT<render_tiles(true)>), 1));
+	CU(set_smem((const void*)k_render_fused<false, false, true>, sizeof(RenderSmemT<render_tiles(false)>), 1));
+	CU(set_smem((const void*)k_render_fused<false, true, true>, sizeof(RenderSmemT<render_tiles(false)>), 1));
+	CU(set_smem((const void*)k_render_fused<false, false, false>, sizeof(RenderSmemT<render_tiles(false)>), 1));
+	CU(set_smem((const void*)k_render_fused<false, true, false>, sizeof(RenderSmemT<render_tiles(false)>), 1));
+	CU(set_smem((const void*)k_render_fused<true, false, false>, sizeof(RenderSmemT<render_tiles(true)>), 1));
+	CU(set_smem((const void*)k_render_fused<true, true, false>, sizeof(RenderSmemT<render_tiles(true)>), 1));
 	cudaFuncAttributes fa;
-	CU(cudaFuncGetAttributes(&fa, k_render_fused<false, false>));
+	CU(cudaFuncGetAttributes(&fa, k_render_fused<false, false, true>));
 	const int by_smem_tile = (int)(prop.sharedMemPerMultiprocessor / (sizeof(tc::TileSmem) + 1024));
 	{   // the operator-level kernels: one tile per CTA, residency from registers / shared memory
 		cudaFuncAttributes fi;
@@ -1223,6 +1202,7 @@ static NsbStatus upload_model_impl(NsbContext* c, const NsbModelDesc* desc, cons
 	}
 	c->model = m;
 	c->desc = *desc;
+	c->dense_in_range = dense_in_range(m.levels, m.n_levels);
 	c->has_model = true;
 	return NSB_OK;
 }
@@ -1750,6 +1730,13 @@ static NsbStatus to_dev_frame(const NsbFrame* f, DevFrame* d) {
 	return NSB_OK;
 }
 
+// The frame's render AABB lies inside its train AABB (a NaN bound fails the test).
+static bool render_in_range(const DevFrame& f) {
+	for (int a = 0; a < 3; ++a)
+		if (!(f.rmin[a] >= f.tmin[a] && f.rmax[a] <= f.tmax[a])) return false;
+	return true;
+}
+
 extern "C" NsbStatus nsb_render(NsbContext* c, const NsbFrame* frame, float* fb_dev, float* depth_dev, void* stream_) {
 	if (!c || !fb_dev || !depth_dev) return fail(NSB_ERR_INVALID, "null argument");
 	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_upload_model has not been called");
@@ -1796,7 +1783,14 @@ extern "C" NsbStatus nsb_render(NsbContext* c, const NsbFrame* frame, float* fb_
 		const uint32_t tiles = (uint32_t)render_tiles(ops_on);
 		uint32_t grid = (uint32_t)c->sm_count;  // one CTA per SM
 		if (grid > (my_tiles + tiles - 1) / tiles) grid = (my_tiles + tiles - 1) / tiles;
-		auto kernel = ops_on ? (c->acc16 ? k_render_fused<true, true> : k_render_fused<true, false>) : (c->acc16 ? k_render_fused<false, true> : k_render_fused<false, false>);
+		// The in-range grid index (nsb_device.cuh) is exact for this frame when render_in_range holds. Without operators the fused kernel
+		// encodes only march samples, and the march hands out only positions inside the render AABB (box_contains). With the render AABB
+		// inside the train AABB, warp_position and warp_position_pow2 (both monotone) map every such position into [0, 1] up to rounding,
+		// well inside [-0.5/scale, 1 + 0.5/scale]. So every grid coordinate is at most res, and dense_in_range bounds the dense index by 2*size.
+		const bool in_range = !ops_on && c->dense_in_range && render_in_range(f);
+		auto kernel = ops_on ? (c->acc16 ? k_render_fused<true, true, false> : k_render_fused<true, false, false>)
+		                     : in_range ? (c->acc16 ? k_render_fused<false, true, true> : k_render_fused<false, false, true>)
+		                                : (c->acc16 ? k_render_fused<false, true, false> : k_render_fused<false, false, false>);
 		kernel<<<grid, 128 * tiles, ops_on ? sizeof(RenderSmemT<render_tiles(true)>) : sizeof(RenderSmemT<render_tiles(false)>), stream>>>(f, c->model, bitfield, c->d_ops.get(), c->n_ops, c->any_poisson,
 		                                                          reinterpret_cast<float4*>(fb_dev), depth_dev, list, ray_od, counters, counters + 1, stats);
 		CU(cudaGetLastError());

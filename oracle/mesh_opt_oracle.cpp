@@ -11,14 +11,6 @@
 
 namespace {
 
-// grid_index of encode_grid
-inline uint32_t grid_entry(const Level& L, const uint32_t* gl) {
-	uint32_t stride = 1, index = 0;
-	for (int dim = 0; dim < 3 && stride <= L.size; ++dim) { index += gl[dim] * stride; stride *= L.res; }
-	if (L.size < stride) index = (gl[0] * 1u) ^ (gl[1] * 2654435761u) ^ (gl[2] * 805459861u);
-	return index % L.size;
-}
-
 // tcnn kernel_grid with prepare_input_gradients (linear interpolation) + kernel_grid_backward_input: dL/dx[d] = the fp32 chain
 // fmaf(float(dfeat_k), dy_dx[k][d], acc) over k = 2l + f ascending, dy_dx[k][d] = the chain over the four corner pairs along d (the other
 // two dims ascending, bit 0 = the lower one) of fmaf(weight, float(v_right) - float(v_left), acc), weight = scale * w_o0 * w_o1; times 1/128.
@@ -31,7 +23,7 @@ void grid_backward(const Model& m, const float* x, const uint16_t* dfeat, float*
 		for (int dim = 0; dim < 3; ++dim) {
 			float p = fmaf(L.scale, x[dim], 0.5f);
 			float fl = floorf(p);
-			gp[dim] = (uint32_t)(int)fl;
+			gp[dim] = (uint32_t)cvt_rzi_s32(fl);
 			w[dim] = p - fl;
 		}
 		for (int d = 0; d < 3; ++d) {
@@ -79,7 +71,7 @@ double density_f64(const Model& m, const double* x, double* grad /* may be null 
 		for (int dim = 0; dim < 3; ++dim) {
 			double p = (double)L.scale * x[dim] + 0.5;
 			double fl = std::floor(p);
-			gp[dim] = (uint32_t)(int64_t)fl;
+			gp[dim] = (uint32_t)cvt_rzi_s32(fl);  // the float64 floor converted as the device converts its float floor
 			w[dim] = p - fl;
 		}
 		feat[2 * l] = feat[2 * l + 1] = 0.0;

@@ -340,15 +340,28 @@ struct Model {
 
 inline uint32_t next_multiple(uint32_t v, uint32_t m) { return ((v + m - 1) / m) * m; }
 
+// The float -> int conversion of tcnn's `(int)floorf(p)` on the GPU, cvt.rzi.s32.f32: truncation toward zero, NaN -> 0, values outside
+// the int range saturate to INT_MIN / INT_MAX. A C++ cast is undefined there (|p| >= 2^31, +-inf, NaN), so the oracle spells it out.
+inline int32_t cvt_rzi_s32(double v) {
+	if (v != v) return 0;
+	if (v >= 2147483648.0) return INT32_MAX;
+	if (v <= -2147483648.0) return INT32_MIN;
+	return (int32_t)v;
+}
+
+// The accepted descriptions: the configs/nerf/base.json topology, log2_hashmap_size 1..24, base_resolution >= 1, per_level_scale >= 1
+// (not NaN), every level's scale below 2^32 (so that `(uint32_t)ceilf(scale) + 1` is defined and fits).
 bool model_init(Model& m, const NsbModelDesc* d, const uint16_t* params, uint64_t n_params) {
 	if (!d || d->n_features_per_level != 2 || d->n_neurons != 64 || d->n_hidden_density != 1 || d->n_hidden_rgb != 2 ||
-	    d->sh_degree != 4 || d->n_levels == 0 || d->n_levels != 16 || d->log2_hashmap_size > 24) return false;
+	    d->sh_degree != 4 || d->n_levels == 0 || d->n_levels != 16 || d->log2_hashmap_size == 0 || d->log2_hashmap_size > 24 ||
+	    d->base_resolution == 0 || !(d->per_level_scale >= 1.0f)) return false;
 	m.desc = *d;
 	m.levels.resize(d->n_levels);
 	float l2s = log2f(d->per_level_scale);
-	uint32_t offset = 0;
+	uint32_t offset = 0;  // at most 16 x 2^24 entries
 	for (uint32_t l = 0; l < d->n_levels; ++l) {
 		float scale = exp2f((float)l * l2s) * (float)d->base_resolution - 1.0f; // grid_scale
+		if (!(scale < 4294967296.0f)) return false;
 		uint32_t res = (uint32_t)ceilf(scale) + 1u;                               // grid_resolution
 		uint32_t max_params = 0xffffffffu / 2;
 		double dense = (double)res * res * res;
@@ -378,6 +391,14 @@ bool model_init(Model& m, const NsbModelDesc* d, const uint16_t* params, uint64_
 	return true;
 }
 
+// tcnn grid_index: the uint32 stride loop (it may wrap), hash where size < stride, then `index % size` on the uint32 index.
+inline uint32_t grid_entry(const Level& L, const uint32_t* gl) {
+	uint32_t stride = 1, index = 0;
+	for (int dim = 0; dim < 3 && stride <= L.size; ++dim) { index += gl[dim] * stride; stride *= L.res; }
+	if (L.size < stride) index = (gl[0] * 1u) ^ (gl[1] * 2654435761u) ^ (gl[2] * 805459861u);
+	return index % L.size;
+}
+
 // tcnn kernel_grid<__half,3,2>, linear interpolation: out[l*2+f], fp16.
 void encode_grid(const Model& m, V3 x, uint16_t* out /*32*/) {
 	const float xin[3] = {x.x, x.y, x.z};
@@ -388,7 +409,7 @@ void encode_grid(const Model& m, V3 x, uint16_t* out /*32*/) {
 		for (int dim = 0; dim < 3; ++dim) { // pos_fract
 			float p = fmaf(L.scale, xin[dim], 0.5f);
 			float fl = floorf(p);
-			g[dim] = (uint32_t)(int)fl;
+			g[dim] = (uint32_t)cvt_rzi_s32(fl);
 			w[dim] = p - fl;
 		}
 		uint16_t acc[2] = {0, 0};
@@ -399,12 +420,7 @@ void encode_grid(const Model& m, V3 x, uint16_t* out /*32*/) {
 				if ((idx & (1u << dim)) == 0) { weight *= 1.0f - w[dim]; gl[dim] = g[dim]; }
 				else { weight *= w[dim]; gl[dim] = g[dim] + 1u; }
 			}
-			// grid_index
-			uint32_t stride = 1, index = 0;
-			for (int dim = 0; dim < 3 && stride <= L.size; ++dim) { index += gl[dim] * stride; stride *= L.res; }
-			if (L.size < stride) index = (gl[0] * 1u) ^ (gl[1] * 2654435761u) ^ (gl[2] * 805459861u);
-			index %= L.size;
-			const uint16_t* e = m.grid + ((uint64_t)L.offset + index) * 2;
+			const uint16_t* e = m.grid + ((uint64_t)L.offset + grid_entry(L, gl)) * 2;
 			for (int f = 0; f < 2; ++f) acc[f] = hadd(acc[f], f2h(weight * h2f(e[f]))); // result += (T)(weight*data)
 		}
 		out[l * 2 + 0] = acc[0];
@@ -927,6 +943,15 @@ int orc_level_table(const NsbModelDesc* d, float* scale, uint32_t* res, uint32_t
 	for (uint32_t l = 0; l < d->n_levels; ++l) { scale[l] = m.levels[l].scale; res[l] = m.levels[l].res; offset[l] = m.levels[l].offset; size[l] = m.levels[l].size; }
 	return 0;
 }
+
+// tcnn's grid_index on one level for n grid coordinates g (n x 3): the uint32 index into the level; 1 for a rejected description or level
+int orc_grid_index(const NsbModelDesc* d, uint32_t level, const uint32_t* g, uint32_t n, uint32_t* out) {
+	Model m;
+	if (!model_init(m, d, nullptr, 0) || level >= d->n_levels) return 1;
+	for (uint32_t i = 0; i < n; ++i) out[i] = grid_entry(m.levels[level], g + 3 * (size_t)i);
+	return 0;
+}
+int32_t orc_f2i(float v) { return cvt_rzi_s32(v); }
 
 uint16_t orc_f2h(float f) { return f2h(f); }
 float orc_h2f(uint16_t h) { return h2f(h); }

@@ -60,6 +60,9 @@ def lib() -> C.CDLL:
         l.orc_cascaded_grid_idx_at.argtypes = [C.c_float] * 3 + [C.c_uint32]
         l.orc_model_n_params.argtypes = [C.POINTER(abi.NsbModelDesc), C.POINTER(C.c_uint64)]
         l.orc_level_table.argtypes = [C.POINTER(abi.NsbModelDesc)] + [C.c_void_p] * 4
+        l.orc_grid_index.argtypes = [C.POINTER(abi.NsbModelDesc), C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
+        l.orc_f2i.restype = C.c_int32
+        l.orc_f2i.argtypes = [C.c_float]
         l.orc_encode.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_uint32, C.c_void_p]
         l.orc_inference.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_uint32, C.c_void_p, C.c_int]
         l.orc_map_rays.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_void_p, C.c_uint32]

@@ -83,26 +83,38 @@ def test_level_table_matches_survey_numbers():
     assert np.allclose(s2, scale, rtol=1e-6)
 
 
-def _numpy_encode(model, coords):
-    """Independent restatement of the tcnn hash grid in numpy: float32 weights, fp16 accumulation."""
-    scale, res, offset, size, _ = syn.level_table(model.desc)
+def _f2i_rz_sat(v):
+    """cvt.rzi.s32.f32 as uint32: truncation, NaN -> 0, saturation to the int range, then the two's-complement bits."""
+    v = np.asarray(v, np.float64)
+    v = np.where(np.isnan(v), 0.0, np.clip(v, -2.0 ** 31, 2.0 ** 31 - 1))
+    return np.trunc(v).astype(np.int64).astype(np.uint32)
+
+
+def _numpy_encode(model, coords, desc=None, grid=None):
+    """Independent restatement of the tcnn hash grid in numpy: float32 weights, fp16 accumulation. Total on float32 inputs:
+    coordinates wrap through uint32, the index is `% size` on the uint32 value, and hash vs. dense follows tcnn's uint32 stride."""
+    desc = model.desc if desc is None else desc
+    grid = (model.grid if grid is None else grid).reshape(-1, 2)
+    scale, res, offset, size, _ = syn.level_table(desc)
     # take the level scales from the oracle (libm exp2f bits), everything else is recomputed here
-    L = model.desc.n_levels
+    L = desc.n_levels
     sc = np.zeros(L, np.float32)
     tmp = [np.zeros(L, np.uint32) for _ in range(3)]
-    orc.lib().orc_level_table(C.byref(model.desc), sc.ctypes.data, *[t.ctypes.data for t in tmp])
-    grid = model.grid.reshape(-1, 2)
+    assert orc.lib().orc_level_table(C.byref(desc), sc.ctypes.data, *[t.ctypes.data for t in tmp]) == 0
     x = coords[:, :3].astype(np.float32)
     out = np.zeros((32, x.shape[0]), np.float16)
     for l in range(L):
-        p = (sc[l] * x + np.float32(0.5)).astype(np.float32)  # products < 2^12: a*b+0.5 needs an fma to match bit-exactly
-        p = np.float32(np.float64(sc[l]) * x.astype(np.float64) + 0.5)  # fma == exact product + add, one rounding
-        g = np.floor(p)
-        w = (p - g).astype(np.float32)
-        g = g.astype(np.uint32)
+        with np.errstate(invalid="ignore", over="ignore"):
+            p = np.float32(np.float64(sc[l]) * x.astype(np.float64) + 0.5)  # fma == exact product + add, one rounding
+            g = np.floor(p)
+            w = (p - g).astype(np.float32)
+        g = _f2i_rz_sat(g)
         acc = np.zeros((x.shape[0], 2), np.float16)
         r, n = np.uint32(res[l]), int(size[l])
-        hashed = int(res[l]) ** 3 > n
+        stride, dim = 1, 0
+        while dim < 3 and stride <= n:
+            stride, dim = (stride * int(res[l])) & 0xFFFFFFFF, dim + 1
+        hashed = n < stride
         for c in range(8):
             wt = np.ones(x.shape[0], np.float32)
             gi = []
@@ -113,15 +125,16 @@ def _numpy_encode(model, coords):
                 else:
                     wt = (wt * (np.float32(1.0) - w[:, d])).astype(np.float32)
                     gi.append(g[:, d])
-            if hashed:
-                with np.errstate(over="ignore"):
+            with np.errstate(over="ignore"):
+                if hashed:
                     idx = gi[0] ^ (gi[1] * np.uint32(2654435761)) ^ (gi[2] * np.uint32(805459861))
-            else:
-                idx = gi[0] + gi[1] * r + gi[2] * r * r
+                else:
+                    idx = gi[0] + gi[1] * r + gi[2] * (r * r)  # uint32 arithmetic: wraps like tcnn's
             idx = idx % np.uint32(n)
             vals = grid[int(offset[l]) + idx.astype(np.int64)].astype(np.float32)
-            prod = (wt[:, None] * vals).astype(np.float32).astype(np.float16)
-            acc = (acc.astype(np.float64) + prod.astype(np.float64)).astype(np.float16)  # exact sum, one rounding
+            with np.errstate(invalid="ignore", over="ignore"):
+                prod = (wt[:, None] * vals).astype(np.float32).astype(np.float16)
+                acc = (acc.astype(np.float64) + prod.astype(np.float64)).astype(np.float16)  # exact sum, one rounding
         out[2 * l], out[2 * l + 1] = acc[:, 0], acc[:, 1]
     return out
 
