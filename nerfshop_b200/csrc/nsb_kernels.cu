@@ -162,18 +162,16 @@ __device__ __forceinline__ float h_hi(uint32_t packed) { return __half2float(__u
 // Per-slot ray state parked in shared memory (SoA: lane-contiguous, conflict-free). Only the acquire and composite phases
 // touch it, so it does not occupy registers while the thread gathers hash-grid features and walks the MLP layers.
 enum { R_OX = 0, R_OY, R_OZ, R_DX, R_DY, R_DZ, R_T, R_CR, R_CG, R_CB, R_CA, R_DEPTH, R_MAXW, R_FIELDS };
-// One CTA per SM holds RENDER_TILES independent tiles (a tile = 128 threads = 128 ray slots = one warpgroup). The tiles share the 20 KB
-// weight image — four separate CTAs would hold four copies — which matters because shared memory is carved out of the same
+// One CTA per SM holds render_tiles(OPS, ACC16) independent tiles (a tile = 128 threads = 128 ray slots = one warpgroup). The tiles share
+// the 20 KB weight image — four separate CTAs would hold four copies — which matters because shared memory is carved out of the same
 // 256 KB as the L1 that serves the hash-grid gathers.
-// How many: the register file's worth. Frames without operators: 6 tiles (24 warps per SM, 80 registers per thread, 155 KB of shared memory);
-// the default fp16-accumulator build does not spill, the fp32 one spills 50 B per thread. Frames with operators carry the deform / membrane
-// state: 5 tiles (96 registers; 110-134 B spilled per thread with the wgmma layer chain). Other tile counts are not measured on the H100.
-constexpr int RENDER_TILES = 6, RENDER_TILES_OPS = 5;
+// How many: the register file's worth, per instantiation. Frames without operators and fp16 accumulators (the default): 7 tiles (28 warps
+// per SM, 72 registers per thread, 122 KB of shared memory), no spills. fp32 accumulators: 6 tiles (80 registers, 20 B of spill stores
+// per thread; capped at 72 they spill 66-106 B and ptxas serialises the wgmma chain). Frames with operators carry the deform / membrane
+// state: 5 tiles (96 registers; 86-98 B of spill stores per thread; six tiles at 80 registers spill twice that and measured slower).
+constexpr int RENDER_TILES_ACC16 = 7, RENDER_TILES = 6, RENDER_TILES_OPS = 5;
 struct TileBlock {
-	union {
-		uint8_t a64[tc::A64_BYTES];
-		uint8_t a32[tc::A32_BYTES];
-	};
+	uint8_t a32[tc::A32_BYTES];  // run_network's operand space
 	float ray[R_FIELDS][128];
 };
 template <int TILES>
@@ -184,29 +182,29 @@ struct __align__(128) RenderSmemT {
 	uint64_t w_bar;
 	uint32_t pad[2];
 };
-__host__ __device__ constexpr int render_tiles(bool ops) { return ops ? RENDER_TILES_OPS : RENDER_TILES; }
-static_assert(RENDER_TILES >= 1 && RENDER_TILES <= 8 && RENDER_TILES_OPS >= 1 && RENDER_TILES_OPS <= 8, "1..8 tiles (warpgroups) per CTA");
+__host__ __device__ constexpr int render_tiles(bool ops, bool acc16) { return ops ? RENDER_TILES_OPS : acc16 ? RENDER_TILES_ACC16 : RENDER_TILES; }
+static_assert(RENDER_TILES_ACC16 >= 1 && RENDER_TILES_ACC16 <= 8 && RENDER_TILES >= 1 && RENDER_TILES <= 8 && RENDER_TILES_OPS >= 1 && RENDER_TILES_OPS <= 8,
+              "1..8 tiles (warpgroups) per CTA");
 
 // OPS = false: the instantiation for frames without edit operators (f.apply_ops == 0 or no operator uploaded) carries none of the deform /
 // membrane code in its hot loop (the loop has to fit the instruction cache).
 // ACC16: the MLP accumulator policy (nsb_set_mlp_accumulator): fp16 wgmma accumulators, like the reference's wmma __half fragments.
 // IN_RANGE (only with OPS = false): the hash grid takes grid_index's one-subtraction modulo; the host picks it where render_in_range holds.
 template <bool OPS, bool ACC16, bool IN_RANGE>
-__global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(const DevFrame f, const DevModel m, const uint8_t* __restrict__ bitfield,
+__global__ void __launch_bounds__(128 * render_tiles(OPS, ACC16), 1) k_render_fused(const DevFrame f, const DevModel m, const uint8_t* __restrict__ bitfield,
                                                       const DevOp* __restrict__ ops, const int n_ops, const int any_poisson,
                                                       float4* __restrict__ fb, float* __restrict__ depth_out, const RayRec* __restrict__ list,
                                                       const float* __restrict__ ray_od, const uint32_t* __restrict__ n_queued_ptr, uint32_t* fetch_counter,
                                                       unsigned long long* __restrict__ stats) {
 	extern __shared__ __align__(128) uint8_t smem_raw[];
-	constexpr int TILES = render_tiles(OPS);
+	constexpr int TILES = render_tiles(OPS, ACC16);
 	using RenderSmem = RenderSmemT<TILES>;
 	RenderSmem& RS = *reinterpret_cast<RenderSmem*>(smem_raw);
 	const uint32_t tid = threadIdx.x & 127u;      // slot / row within the tile
 	const uint32_t tile = threadIdx.x >> 7;
 	TileBlock& TB = RS.tile[tile];
 	const uint32_t lane = tid & 31u;
-	const uint32_t n_queued = *n_queued_ptr;
-	if (blockIdx.x * 128u * TILES >= n_queued && blockIdx.x > 0) return;  // nothing this CTA could ever fetch
+	if (blockIdx.x * 128u * TILES >= *n_queued_ptr && blockIdx.x > 0) return;  // nothing this CTA could ever fetch
 
 	// CTA setup: one bulk-TMA copy of the weight image
 	tc::load_weights(RS.w, &RS.w_bar, m.w_image);
@@ -275,6 +273,8 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS), 1) k_render_fused(con
 				const unsigned alive_m = __ballot_sync(0xffffffffu, alive);
 				const unsigned want = exhausted ? 0u : ~alive_m;
 				if (want && __popc(alive_m) <= REFILL_THR) {
+					// read at each refill (an L1 hit), not held across the round: at 72 registers a held copy is spilled
+					const uint32_t n_queued = __ldca(n_queued_ptr);
 					const uint32_t need = (uint32_t)__popc(want), rank = (uint32_t)__popc(want & ((1u << lane) - 1u));
 					uint32_t base = 0;
 					if (lane == 0) base = atomicAdd(fetch_counter, need);
@@ -1099,16 +1099,16 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 		if (pct > 100) pct = 100;
 		return cudaFuncSetAttribute(func, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
 	};
-	// k_render_fused: ONE CTA of RENDER_TILES (RENDER_TILES_OPS with operators) tiles per SM (768 x 80 / 640 x 96 registers = the register file;
-	// shared memory 20 KB weights + 22.5 KB per tile).
-	CU(set_smem((const void*)k_render_fused<false, false, true>, sizeof(RenderSmemT<render_tiles(false)>), 1));
-	CU(set_smem((const void*)k_render_fused<false, true, true>, sizeof(RenderSmemT<render_tiles(false)>), 1));
-	CU(set_smem((const void*)k_render_fused<false, false, false>, sizeof(RenderSmemT<render_tiles(false)>), 1));
-	CU(set_smem((const void*)k_render_fused<false, true, false>, sizeof(RenderSmemT<render_tiles(false)>), 1));
-	CU(set_smem((const void*)k_render_fused<true, false, false>, sizeof(RenderSmemT<render_tiles(true)>), 1));
-	CU(set_smem((const void*)k_render_fused<true, true, false>, sizeof(RenderSmemT<render_tiles(true)>), 1));
+	// k_render_fused: ONE CTA of render_tiles(OPS, ACC16) tiles per SM (896 x 72 / 768 x 80 / 640 x 96 registers = the register file;
+	// shared memory 20 KB weights + 14.5 KB per tile).
+	CU(set_smem((const void*)k_render_fused<false, false, true>, sizeof(RenderSmemT<render_tiles(false, false)>), 1));
+	CU(set_smem((const void*)k_render_fused<false, true, true>, sizeof(RenderSmemT<render_tiles(false, true)>), 1));
+	CU(set_smem((const void*)k_render_fused<false, false, false>, sizeof(RenderSmemT<render_tiles(false, false)>), 1));
+	CU(set_smem((const void*)k_render_fused<false, true, false>, sizeof(RenderSmemT<render_tiles(false, true)>), 1));
+	CU(set_smem((const void*)k_render_fused<true, false, false>, sizeof(RenderSmemT<render_tiles(true, false)>), 1));
+	CU(set_smem((const void*)k_render_fused<true, true, false>, sizeof(RenderSmemT<render_tiles(true, true)>), 1));
 	cudaFuncAttributes fa;
-	CU(cudaFuncGetAttributes(&fa, k_render_fused<false, false, true>));
+	CU(cudaFuncGetAttributes(&fa, k_render_fused<false, true, true>));
 	const int by_smem_tile = (int)(prop.sharedMemPerMultiprocessor / (sizeof(tc::TileSmem) + 1024));
 	{   // the operator-level kernels: one tile per CTA, residency from registers / shared memory
 		cudaFuncAttributes fi;
@@ -1136,8 +1136,9 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 			CU(set_smem(f, sizeof(meshopt::GradSmem), c->inference_ctas_per_sm));
 	}
 	if (getenv("NSB_VERBOSE"))
-		fprintf(stderr, "[nsb] device %d: %d SMs; k_render_fused %d tiles/CTA (%d with operators), %d regs, %zu B smem; inference %d CTAs/SM, grid update %d CTAs/SM\n", device, c->sm_count,
-		        render_tiles(false), render_tiles(true), fa.numRegs, sizeof(RenderSmemT<render_tiles(false)>), c->inference_ctas_per_sm, c->grid_update_ctas_per_sm);
+		fprintf(stderr, "[nsb] device %d: %d SMs; k_render_fused %d tiles/CTA (%d with fp32 accumulators, %d with operators), %d regs, %zu B smem; inference %d CTAs/SM, grid update %d CTAs/SM\n",
+		        device, c->sm_count, render_tiles(false, true), render_tiles(false, false), render_tiles(true, true), fa.numRegs, sizeof(RenderSmemT<render_tiles(false, true)>),
+		        c->inference_ctas_per_sm, c->grid_update_ctas_per_sm);
 	*out = c.release();
 	return NSB_OK;
 }
@@ -1780,7 +1781,7 @@ extern "C" NsbStatus nsb_render(NsbContext* c, const NsbFrame* frame, float* fb_
 		CU(cudaGetLastError());
 		CU(cudaEventRecord(c->evm, stream));
 		const bool ops_on = f.apply_ops && c->n_ops > 0;
-		const uint32_t tiles = (uint32_t)render_tiles(ops_on);
+		const uint32_t tiles = (uint32_t)render_tiles(ops_on, c->acc16);
 		uint32_t grid = (uint32_t)c->sm_count;  // one CTA per SM
 		if (grid > (my_tiles + tiles - 1) / tiles) grid = (my_tiles + tiles - 1) / tiles;
 		// The in-range grid index (nsb_device.cuh) is exact for this frame when render_in_range holds. Without operators the fused kernel
@@ -1791,7 +1792,9 @@ extern "C" NsbStatus nsb_render(NsbContext* c, const NsbFrame* frame, float* fb_
 		auto kernel = ops_on ? (c->acc16 ? k_render_fused<true, true, false> : k_render_fused<true, false, false>)
 		                     : in_range ? (c->acc16 ? k_render_fused<false, true, true> : k_render_fused<false, false, true>)
 		                                : (c->acc16 ? k_render_fused<false, true, false> : k_render_fused<false, false, false>);
-		kernel<<<grid, 128 * tiles, ops_on ? sizeof(RenderSmemT<render_tiles(true)>) : sizeof(RenderSmemT<render_tiles(false)>), stream>>>(f, c->model, bitfield, c->d_ops.get(), c->n_ops, c->any_poisson,
+		const size_t smem = ops_on ? sizeof(RenderSmemT<render_tiles(true, false)>)
+		                           : c->acc16 ? sizeof(RenderSmemT<render_tiles(false, true)>) : sizeof(RenderSmemT<render_tiles(false, false)>);
+		kernel<<<grid, 128 * tiles, smem, stream>>>(f, c->model, bitfield, c->d_ops.get(), c->n_ops, c->any_poisson,
 		                                                          reinterpret_cast<float4*>(fb_dev), depth_dev, list, ray_od, counters, counters + 1, stats);
 		CU(cudaGetLastError());
 	}

@@ -37,8 +37,8 @@ constexpr uint32_t W4_OFF = W3_OFF + 64 * 32 * 2;
 constexpr uint32_t W5_OFF = W4_OFF + 64 * 64 * 2;
 constexpr uint32_t W_BYTES = W5_OFF + 16 * 64 * 2;  // 20480
 
-// Operand space of a tile: chunks 0-3 = the 32-wide layer input (grid features for L1; density output + SH for L3), chunks 4-5 =
-// the hand-back of the rgb output. The a32 view aliases the first half of a64.
+// Operand space of a one-tile CTA: chunks 0-3 = the 32-wide layer input (grid features for L1; density output + SH for L3), all that
+// run_network uses; k_density_gradient hands its density output back through chunk 6. The a32 view aliases the first half of a64.
 struct __align__(128) TileSmem {
 	uint8_t w[W_BYTES];
 	union {
@@ -236,7 +236,7 @@ __device__ __forceinline__ void layer_rs(uint32_t* d, const uint32_t* x, uint32_
 // ---- a tile = 128 threads (one warpgroup) walking the layer chain together. A CTA may hold several tiles
 // (they share the weight image; each has its own operand space and named barrier).
 struct TileCtx {
-	uint8_t* a32;        // operand space (A64_BYTES); the 32-wide operand is its first half
+	uint8_t* a32;        // operand space (A32_BYTES): the 32-wide layer input
 	uint32_t w_addr;     // shared-window address of the weight image
 	uint32_t row;        // sample 0..127 within the tile
 	uint32_t bar_id;     // named barrier of the tile (0 = the CTA barrier when the CTA is one tile)
@@ -290,8 +290,11 @@ __device__ __forceinline__ void store_out16(uint8_t* base, uint32_t chunk, uint3
 //   density_only: stop after L2 (NerfNetwork::density)
 //   dens[8]: the 16 fp16 outputs of the density MLP (packed half2), rgb[8]: the 16 outputs of the rgb MLP, both for sample c.row.
 // `dw` = this sample's warped view direction; its 16 SH values are evaluated between L2 and L3.
-// Operand space: chunks 0-3 the 32-wide layer inputs, 4-5 the rgb hand-back, 6-7 the density hand-back. On return the whole tile has
-// finished with the operand space, so the caller may overwrite any of it.
+// Operand space: chunks 0-3, the 32-wide layer input (A32_BYTES). A half's 16-wide output goes back to its owning threads through
+// chunks 0-1 of that half's own rows: the half's first layer (L1 or L3) has returned from layer_ss, and each of those rows is read only
+// by the warp that writes it (phys_row), which has waited on that wgmma, so the rows are free. The density output left there is the rgb
+// network's input columns 0-15 byte for byte. On return the whole tile has finished with the operand space, so the caller may
+// overwrite any of it.
 template <bool ACC16 = false>
 __device__ __forceinline__ void run_network(const TileCtx& c, V3 dw, bool density_only, uint32_t* dens, uint32_t* rgb) {
 	const uint32_t row = c.row;
@@ -304,20 +307,22 @@ __device__ __forceinline__ void run_network(const TileCtx& c, V3 dw, bool densit
 		Acc<16, ACC16> o;
 		layer_ss<64, 32, ACC16>(x.r, a32 + h * 64 * 16, w + W1_OFF);      // L1: grid features (32) -> 64
 		layer_rs<16, 64, ACC16>(o.r, x.r, w + W2_OFF);                    // L2: 64 -> 16
-		store_out16<ACC16>(c.a32, 6, row, h, o.r);
+		store_out16<ACC16>(c.a32, 0, row, h, o.r);
 	}
 	__syncwarp();
 	{
-		const uint4 d0 = load_chunk(c.a32, 6, row), d1 = load_chunk(c.a32, 7, row);
+		const uint4 d0 = load_chunk(c.a32, 0, row), d1 = load_chunk(c.a32, 1, row);
 		dens[0] = d0.x; dens[1] = d0.y; dens[2] = d0.z; dens[3] = d0.w; dens[4] = d1.x; dens[5] = d1.y; dens[6] = d1.z; dens[7] = d1.w;
 	}
-	tile_sync(c);  // every warp's first layer has read its operand
-	if (density_only) return;
-	// rgb-network input: columns 0-15 = density MLP output, 16-31 = SH (nerf_network_full.h:52,67,79)
+	if (density_only) {
+		tile_sync(c);
+		return;
+	}
+	// rgb-network input: columns 0-15 = density MLP output (already in chunks 0-1), 16-31 = SH (nerf_network_full.h:52,67,79).
+	// No tile barrier before the SH stores: they go to this thread's own rows, which only this warp's L1 wgmma ops read, and this warp
+	// has waited on both of them.
 	__half2 sh[8];
 	encode_sh4(dw, sh);  // tcnn SphericalHarmonics of the (mapped) direction
-	store_chunk(c.a32, 0, row, make_uint4(dens[0], dens[1], dens[2], dens[3]));
-	store_chunk(c.a32, 1, row, make_uint4(dens[4], dens[5], dens[6], dens[7]));
 	store_chunk(c.a32, 2, row, make_uint4(pack_h2(sh[0]), pack_h2(sh[1]), pack_h2(sh[2]), pack_h2(sh[3])));
 	store_chunk(c.a32, 3, row, make_uint4(pack_h2(sh[4]), pack_h2(sh[5]), pack_h2(sh[6]), pack_h2(sh[7])));
 	fence_async_smem();
@@ -329,11 +334,11 @@ __device__ __forceinline__ void run_network(const TileCtx& c, V3 dw, bool densit
 		layer_ss<64, 32, ACC16>(x.r, a32 + h * 64 * 16, w + W3_OFF);  // L3: 32 -> 64
 		layer_rs<64, 64, ACC16>(y.r, x.r, w + W4_OFF);                // L4: 64 -> 64
 		layer_rs<16, 64, ACC16>(o.r, y.r, w + W5_OFF);                // L5: 64 -> 16
-		store_out16<ACC16>(c.a32, 4, row, h, o.r);
+		store_out16<ACC16>(c.a32, 0, row, h, o.r);
 	}
 	__syncwarp();
 	{
-		const uint4 r0 = load_chunk(c.a32, 4, row), r1 = load_chunk(c.a32, 5, row);
+		const uint4 r0 = load_chunk(c.a32, 0, row), r1 = load_chunk(c.a32, 1, row);
 		rgb[0] = r0.x; rgb[1] = r0.y; rgb[2] = r0.z; rgb[3] = r0.w; rgb[4] = r1.x; rgb[5] = r1.y; rgb[6] = r1.z; rgb[7] = r1.w;
 	}
 	tile_sync(c);
