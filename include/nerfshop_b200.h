@@ -255,8 +255,9 @@ NsbStatus nsb_host_frame_wait(NsbContext* ctx, uint64_t ticket);
 /* Synchronises and returns the counters of the last render. */
 NsbStatus nsb_get_stats(NsbContext* ctx, NsbRenderStats* out);
 
-/* Diagnostics of the last nsb_render (not part of the reference surface): out[0..6] = MLP rounds summed over CTAs, and
- * per-phase SM cycles of one thread per CTA summed over CTAs {acquire/march, encode, mlp, composite, total}, CTAs run. */
+/* Diagnostics of the last nsb_render (not part of the reference surface), counted per render tile (128 threads; a CTA of the
+ * fused renderer holds 5-7 of them): out[0..6] = MLP rounds summed over tiles, per-phase SM cycles of thread 0 of each tile summed
+ * over tiles {acquire/march, encode, mlp, composite, total}, tiles run. */
 NsbStatus nsb_debug_counters(NsbContext* ctx, uint64_t* out, int32_t n);
 
 /* Multi-GPU helpers: packed tile buffers for the single framebuffer gather.

@@ -31,7 +31,7 @@ using namespace nsb;
 struct RayRec { uint32_t pix; float t; };  // a ray that entered the AABB and found occupied space: pixel + first sample t
 
 enum { ST_RAYS = 0, ST_ALIVE = 1, ST_HIT = 2, ST_SAMPLES = 3, ST_OLD = 4, ST_ROUNDS = 5, ST_CYC_ACQUIRE = 6, ST_CYC_ENCODE = 7, ST_CYC_MLP = 8,
-       ST_CYC_COMPOSITE = 9, ST_CYC_TOTAL = 10, ST_CTAS = 11, ST_N = 12 };
+       ST_CYC_COMPOSITE = 9, ST_CYC_TOTAL = 10, ST_TILES = 11, ST_N = 12 };
 constexpr int DDA_BUDGET = 8;   // empty voxels a lane may skip per MLP round before it yields (latency bound of a round)
 constexpr int REFILL_THR = 2;   // the free lanes of a warp refill once at most this many of its rays are alive
 
@@ -222,8 +222,8 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS, ACC16), 1) k_render_fu
 	bool alive = false, exhausted = false;  // exhausted is warp-uniform: the queue had nothing left when this warp last asked
 	uint32_t pix = 0, n_steps = 0;
 	uint32_t c_hit = 0, c_samples = 0, c_old = 0;
-	// phase profile (thread 0 of each CTA; a handful of clock reads per round): diagnostic builds only (-DNSB_PROFILE), the
-	// product build keeps the registers and issue slots (nsb_debug_counters then reports rounds and CTAs only)
+	// phase profile (thread 0 of each tile; a handful of clock reads per round): diagnostic builds only (-DNSB_PROFILE), the
+	// product build keeps the registers and issue slots (nsb_debug_counters then reports rounds and tiles only)
 #ifdef NSB_PROFILE
 #define NSB_CLOCK() clock64()
 	long long cyc_acq = 0, cyc_enc = 0, cyc_mlp = 0, cyc_comp = 0;
@@ -500,7 +500,7 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS, ACC16), 1) k_render_fu
 		atomicAdd(stats + ST_CYC_COMPOSITE, (unsigned long long)cyc_comp);
 		atomicAdd(stats + ST_CYC_TOTAL, (unsigned long long)(clock64() - cyc_start));
 #endif
-		atomicAdd(stats + ST_CTAS, 1ull);
+		atomicAdd(stats + ST_TILES, 1ull);
 	}
 
 	// counters: warp reduce, one atomic per warp
@@ -1883,8 +1883,8 @@ extern "C" NsbStatus nsb_get_stats(NsbContext* c, NsbRenderStats* out) {
 	return NSB_OK;
 }
 
-// Diagnostic counters of the last render: rounds (CTA x MLP rounds), and thread-0 cycles per phase summed over CTAs:
-// {rounds, acquire, encode, mlp, composite, total, ctas}
+// Diagnostic counters of the last render, per render tile (thread 0 of each 128-thread tile adds them): rounds (tile x MLP rounds),
+// and cycles per phase summed over tiles: {rounds, acquire, encode, mlp, composite, total, tiles}
 extern "C" NsbStatus nsb_debug_counters(NsbContext* c, uint64_t* out, int32_t n) {
 	if (!c || !out || n < 7) return fail(NSB_ERR_INVALID, "need room for 7 counters");
 	CU(cudaSetDevice(c->device));

@@ -204,7 +204,7 @@ class NerfRenderer:
     def debug_counters(self) -> dict:
         out = (C.c_uint64 * 7)()
         abi.check(self.lib, self.lib.nsb_debug_counters(self.ctx, out, 7), "nsb_debug_counters")
-        keys = ("rounds", "cyc_acquire", "cyc_encode", "cyc_mlp", "cyc_composite", "cyc_total", "ctas")
+        keys = ("rounds", "cyc_acquire", "cyc_encode", "cyc_mlp", "cyc_composite", "cyc_total", "tiles")  # summed over / counting render tiles
         return dict(zip(keys, [int(v) for v in out]))
 
     # ---- multi-GPU framebuffer shards ------------------------------------------------------------------

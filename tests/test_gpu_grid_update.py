@@ -19,6 +19,7 @@ from test_grid_update_cpu import grid_params
 pytestmark = pytest.mark.gpu
 
 RTOL = 4 * 2.0 ** -7
+POLICIES = {"f16": (abi.NSB_MLP_ACC_F16, 1), "f32": (abi.NSB_MLP_ACC_F32, 0)}  # device policy (nsb_set_mlp_accumulator), oracle policy
 
 
 def _compare(g_gpu, b_gpu, g_cpu, b_cpu, mean_cpu):
@@ -42,13 +43,23 @@ def _compare(g_gpu, b_gpu, g_cpu, b_cpu, mean_cpu):
 
 
 def test_grid_update_no_operators(scene, renderer):
+    _grid_update_no_operators(scene, renderer, "f16")
+
+
+def test_grid_update_no_operators_fp32_accumulators(scene, renderer):
+    _grid_update_no_operators(scene, renderer, "f32")
+
+
+def _grid_update_no_operators(scene, renderer, policy):
     model, occ = scene
     o = orc.Oracle(model.desc, model.params, occ)
     rng = Pcg32(1337)
     rng_o = rng.copy()
     g_cpu = np.zeros(abi.NSB_GRID_CELLS, np.float32)
     state = {"rng": rng, "ema_step": 0}
+    old = orc.set_mlp_policy(POLICIES[policy][1])
     try:
+        renderer.set_mlp_accumulator(POLICIES[policy][0])
         for step, (nu, nn, reset) in enumerate([(600_000, 0, True), (300_000, 200_000, False)]):
             u = grid_params(nu, nn, rng_o, ema_step=step, reset=reset)
             g_cpu, b_cpu, mean = o.update_density_grid(u, g_cpu)
@@ -57,31 +68,38 @@ def test_grid_update_no_operators(scene, renderer):
             state["ema_step"] += 1
             g_gpu, b_gpu = renderer.download_density_grid()
             exact, rel, nbytes = _compare(g_gpu, b_gpu, g_cpu, b_cpu, mean)
-            print(f"step {step}: {exact:.5f} of touched cells bit-equal, max |ln ratio| {rel:.3g}, {nbytes} bitfield bytes differ")
+            print(f"{policy} step {step}: {exact:.5f} of touched cells bit-equal, max |ln ratio| {rel:.3g}, {nbytes} bitfield bytes differ")
             g_cpu = g_gpu.copy()  # continue both from the same state so the second step's cell selection stays comparable
         assert (state["rng"].state, state["rng"].inc) == (rng_o.state, rng_o.inc)
     finally:
+        orc.set_mlp_policy(old)
+        renderer.set_mlp_accumulator(abi.NSB_MLP_ACC_F16)
         renderer.upload_occupancy(occ)
 
 
+@pytest.mark.parametrize("policy", sorted(POLICIES))
 @pytest.mark.parametrize("fixture", ["e1", "e3"])
-def test_grid_update_through_operators(scene, renderer, fixture):
+def test_grid_update_through_operators(scene, renderer, fixture, policy):
     model, occ = scene
     ops = [op.to_op() for op in getattr(fx, fixture)(model)]
     o = orc.Oracle(model.desc, model.params, occ, ops)
     renderer.set_edit_operators(ops)
+    old = orc.set_mlp_policy(POLICIES[policy][1])
     try:
+        renderer.set_mlp_accumulator(POLICIES[policy][0])
         rng = Pcg32(99)
         u = grid_params(128 ** 3, 0, rng, n_cascades=1)  # every cascade-0 cell index is visited (the index is a bijection mod 128^3)
         g_cpu, b_cpu, mean = o.update_density_grid(u, np.zeros(abi.NSB_GRID_CELLS, np.float32))
         renderer.update_density_grid(rng.copy(), 0, 128 ** 3, 0, reset_grid=True, n_cascades=1)
         g_gpu, b_gpu = renderer.download_density_grid()
         exact, rel, nbytes = _compare(g_gpu, b_gpu, g_cpu, b_cpu, mean)
-        print(f"{fixture}: {exact:.5f} bit-equal, max |ln ratio| {rel:.3g}, {nbytes} bitfield bytes differ")
+        print(f"{fixture} {policy}: {exact:.5f} bit-equal, max |ln ratio| {rel:.3g}, {nbytes} bitfield bytes differ")
         # and the operators did change the grid
         g_plain, _, _ = orc.Oracle(model.desc, model.params, occ).update_density_grid(u, np.zeros(abi.NSB_GRID_CELLS, np.float32))
         assert (g_plain != g_cpu).sum() > 100
     finally:
+        orc.set_mlp_policy(old)
+        renderer.set_mlp_accumulator(abi.NSB_MLP_ACC_F16)
         renderer.reset_edit_operators()
         renderer.upload_occupancy(occ)
 

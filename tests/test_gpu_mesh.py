@@ -2,6 +2,7 @@
 scene over its render AABB [-1.5, 2.5]^3. The running density grid is the occupancy bitfield as 0/1 floats, so the filter is active
 (-10000) on empty cascade cells. Threshold: the median raw density of the unfiltered points, at which the surface is closed (every
 grid point on the box boundary is filtered)."""
+import contextlib
 import ctypes as C
 
 import numpy as np
@@ -53,14 +54,36 @@ def _mesh(mr, res, thresh, shade=True):
     return d.cpu().numpy(), mr.mesh_download(nv, ni, shaded=shade), nv
 
 
+@contextlib.contextmanager
+def _policy(mr, policy):
+    """The accumulator policy ("f16" or "f32", nsb_set_mlp_accumulator) for a block: nsb_density_on_grid and nsb_mesh_shade follow it like
+    nsb_density and nsb_inference. The fp16 default is restored after it."""
+    from nerfshop_b200 import abi
+
+    try:
+        mr.set_mlp_accumulator(abi.NSB_MLP_ACC_F16 if policy == "f16" else abi.NSB_MLP_ACC_F32)
+        yield
+    finally:
+        mr.set_mlp_accumulator(abi.NSB_MLP_ACC_F16)
+
+
 def test_density_on_grid_equals_nsb_density_and_filters_empty_cells(mr, scene):
+    _density_on_grid_equals_nsb_density(mr, scene, "f16")
+
+
+def test_density_on_grid_equals_nsb_density_with_fp32_accumulators(mr, scene):
+    _density_on_grid_equals_nsb_density(mr, scene, "f32")
+
+
+def _density_on_grid_equals_nsb_density(mr, scene, policy):
     res = 64
-    got = _density(mr, res)
     p, pw = _positions(res)
     coords = np.zeros((pw.shape[0], 7), np.float32)
     coords[:, :3] = pw
     coords[:, 4:] = 0.5
-    raw = mr.density(coords)[0].view(np.float16).astype(np.float32)
+    with _policy(mr, policy):
+        got = _density(mr, res)
+        raw = mr.density(coords)[0].view(np.float16).astype(np.float32)
     # cascaded_grid_at(unwarp(warp(p)), density_grid, mip_from_pos) of the occupancy as 0/1: the unwarp is exact here
     from nerfshop_b200 import synthetic as syn
 
@@ -101,10 +124,19 @@ def test_marching_cubes_matches_the_oracle_and_is_deterministic(mr):
 
 
 def test_normals_and_colours(mr):
+    _normals_and_colours(mr, "f16")
+
+
+def test_normals_and_colours_with_fp32_accumulators(mr):
+    _normals_and_colours(mr, "f32")
+
+
+def _normals_and_colours(mr, policy):
     res = 64
-    d0 = _density(mr, res)
-    t = _thresh(d0)
-    d, m, nv = _mesh(mr, res, t)
+    with _policy(mr, policy):
+        d0 = _density(mr, res)
+        t = _thresh(d0)
+        d, m, nv = _mesh(mr, res, t)
     V, N, Cc, F = m["V"], m["N"], m["C"], m["F"].astype(np.int64)
     # normals: (pb - pa) x (pa - pc) per triangle, summed in triangle order; the device contracts the cross product into FMAs, so
     # compare in angle
@@ -122,7 +154,8 @@ def test_normals_and_colours(mr):
     coords = np.zeros((V.shape[0], 7), np.float32)
     coords[:, :3] = (V - np.float32(-1.5)) / np.float32(4.0)
     coords[:, 4:] = (dirs + np.float32(1.0)) * np.float32(0.5)
-    raw = mr.inference(coords)[:3].view(np.float16).astype(np.float32).T
+    with _policy(mr, policy):
+        raw = mr.inference(coords)[:3].view(np.float16).astype(np.float32).T
     same = (raw == Cc).all(1)
     assert same.mean() > 0.99  # direction bits may differ in the last place where float64 rounds differently from the FMA form
     assert np.abs(raw - Cc).max() < 2e-2

@@ -111,6 +111,6 @@ if stage in ("all", "perf"):
     d = r.debug_counters()
     rounds = max(d["rounds"], 1)
     print("debug", d)
-    print(f"  lane utilisation {st.n_samples / (rounds * 128):.3f}; rounds/CTA {rounds / max(d['ctas'], 1):.1f}; cycles/round: acquire {d['cyc_acquire'] / rounds:.0f} encode {d['cyc_encode'] / rounds:.0f} "
-          f"mlp {d['cyc_mlp'] / rounds:.0f} composite {d['cyc_composite'] / rounds:.0f}; total cyc/CTA {d['cyc_total'] / max(d['ctas'], 1):.0f}", flush=True)
+    print(f"  lane utilisation {st.n_samples / (rounds * 128):.3f}; rounds/tile {rounds / max(d['tiles'], 1):.1f}; cycles/round: acquire {d['cyc_acquire'] / rounds:.0f} encode {d['cyc_encode'] / rounds:.0f} "
+          f"mlp {d['cyc_mlp'] / rounds:.0f} composite {d['cyc_composite'] / rounds:.0f}; total cyc/tile {d['cyc_total'] / max(d['tiles'], 1):.0f}", flush=True)
 r.close()
