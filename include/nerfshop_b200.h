@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define NSB_ABI_VERSION 5
+#define NSB_ABI_VERSION 6
 
 /* reference: common_nerf.h:16-39 */
 #define NSB_NERF_GRIDSIZE 128u
@@ -471,6 +471,34 @@ typedef struct {
  * of the positions before the last step. Adam state (48 B per vertex row) is allocated on the first call and restarts with the first call
  * after each nsb_marching_cubes. NSB_ERR_STATE without a model or a mesh. Stream-ordered. */
 NsbStatus nsb_mesh_optimise(NsbContext* ctx, const NsbMeshOptimise* params, uint32_t n_steps, void* stream);
+
+/* ---- density and RGBA slices (ABI 6): the export panel's "Save density PNG" (Testbed::compute_and_save_png_slices, testbed.cu:345-366,
+ * python_api.cu:458) and "Save RGBA PNG sequence" (testbed.cu:956-966). The caller writes the PNG files from the pixels; none of these
+ * calls allocates in the context ------------------------------------------------------------------------------------------------------ */
+/* replaces Testbed::get_rgba_on_grid (testbed_nerf.cu:4588-4612): rgba_dev (DEVICE float4[res_x*res_y*res_z], x fastest, 16-byte aligned)
+ * receives, at the grid positions of nsb_density_on_grid over query->aabb (the reference samples m_render_aabb) seen from direction ray_dir,
+ * compute_nerf_density (:624-635) of the full network's output: a = clamp(1 - exp(-network_to_density(density) / 100), 0, 1) and
+ * rgb = network_to_rgb(rgb) * a, in one pass without the reference's position buffer (28 B per point) or its 1M-point batches. Same res rules
+ * as nsb_density_on_grid; no density grid is needed (the reference applies no filter here). NSB_ERR_STATE without a model. Stream-ordered. */
+NsbStatus nsb_rgba_on_grid(NsbContext* ctx, const NsbGridQuery* query, const float ray_dir[3], int32_t rgb_activation, int32_t density_activation,
+                           float* rgba_dev, void* stream);
+/* The size of save_density_grid_to_png's mosaic (marching_cubes.cu:938-945): with res' = (res_x, res_z, res_y) when swap_y_z, else res,
+ * ndown = (uint32_t)sqrtf(res'_z), nacross = ceil(res'_z / ndown), *w = res_x * nacross, *h = res'_y * ndown. Needs no GPU. */
+NsbStatus nsb_density_png_extent(const int32_t res[3], int32_t swap_y_z, uint32_t* w, uint32_t* h);
+/* replaces the host loops of save_density_grid_to_png (marching_cubes.cu:898-974) on a DEVICE float grid (x fastest; any positive res
+ * with a 32-bit point count), without copying the grid to the host. pixels_dev: DEVICE uint8[w * h] (nsb_density_png_extent), the
+ * bytes the reference hands to stbi_write_png: tile (i, j) shows slice j * nacross + i, pixel (x, y) of it is
+ * (uint8_t)clamp((d - thresh) * (128 / density_range) + 128.5, 0, 255) with the product and sum rounded separately, rows flipped in y
+ * unless swap_y_z; tiles past the last slice are 0. counts_dev: DEVICE uint64[2], the logged #zero-x voxels (cells with corners on both
+ * sides of thresh) and #lattice near zero-x (grid points with a 6-neighbour on the other side), both over the interior grid points
+ * 1 <= x, y, z <= res - 2; integer atomics, so they do not depend on the order. density_range > 0. Needs no model. Stream-ordered. */
+NsbStatus nsb_density_png(NsbContext* ctx, const float* density_dev, const int32_t res[3], float thresh, float density_range, int32_t swap_y_z,
+                          uint8_t* pixels_dev, uint64_t* counts_dev, void* stream);
+/* replaces the host loop of save_rgba_grid_to_png_sequence (marching_cubes.cu:979-1015) on a DEVICE float4 grid (e.g. nsb_rgba_on_grid's,
+ * 16-byte aligned): pixels_dev (DEVICE, 4-byte aligned) receives res'_z images of res_x * res'_y RGBA pixels back to back, slice z being
+ * the reference's file %04d_<w>x<h>.png, each channel (uint8_t)clamp(v * 255, 0, 255); res' and the y flip as nsb_density_png. Needs no
+ * model. Stream-ordered. */
+NsbStatus nsb_rgba_png(NsbContext* ctx, const float* rgba_dev, const int32_t res[3], int32_t swap_y_z, uint8_t* pixels_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libnerfshop_b200.so")
 
-NSB_ABI_VERSION = 5
+NSB_ABI_VERSION = 6
 NSB_MLP_ACC_F32, NSB_MLP_ACC_F16 = 0, 1
 NSB_NERF_GRIDSIZE = 128
 NSB_NERF_CASCADES = 5
@@ -149,6 +149,7 @@ EXPORTED_SYMBOLS = [
     "nsb_build_tet_grid", "nsb_compute_mvc", "nsb_interpolate_with_mvc", "nsb_local_rotations",
     "nsb_density_on_grid", "nsb_marching_cubes", "nsb_mesh_shade", "nsb_mesh_download",
     "nsb_density_gradient", "nsb_mesh_optimise",
+    "nsb_rgba_on_grid", "nsb_density_png_extent", "nsb_density_png", "nsb_rgba_png",
 ]
 
 _lib = None
@@ -224,6 +225,10 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.nsb_mesh_download.argtypes = [vp, vp, vp, vp, u64, vp, u64]
     lib.nsb_density_gradient.argtypes = [vp, vp, u32, vp, u32, vp, vp, u32, vp]
     lib.nsb_mesh_optimise.argtypes = [vp, C.POINTER(NsbMeshOptimise), u32, vp]
+    lib.nsb_rgba_on_grid.argtypes = [vp, C.POINTER(NsbGridQuery), C.POINTER(f32), i32, i32, vp, vp]
+    lib.nsb_density_png_extent.argtypes = [C.POINTER(i32), i32, C.POINTER(u32), C.POINTER(u32)]
+    lib.nsb_density_png.argtypes = [vp, vp, C.POINTER(i32), f32, f32, i32, vp, vp, vp]
+    lib.nsb_rgba_png.argtypes = [vp, vp, C.POINTER(i32), i32, vp, vp]
     for name in EXPORTED_SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("nsb_last_error", "nsb_abi_version"):

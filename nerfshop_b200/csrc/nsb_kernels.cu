@@ -924,6 +924,7 @@ __global__ void k_unpack_gathered(const float4* __restrict__ gathered, const flo
 
 #include "nsb_mesh.cuh"
 #include "nsb_mesh_opt.cuh"
+#include "nsb_slices.cuh"
 
 // =====================================================================================================
 // host side: context, uploads, C ABI
@@ -1129,7 +1130,7 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 		CU(set_smem((const void*)k_density_grid_update<false>, sizeof(tc::TileSmem), c->grid_update_ctas_per_sm));
 		CU(set_smem((const void*)k_density_grid_update<true>, sizeof(tc::TileSmem), c->grid_update_ctas_per_sm));
 		for (const void* f : {(const void*)mesh::k_density_on_grid<false>, (const void*)mesh::k_density_on_grid<true>, (const void*)mesh::k_mesh_colors<false>,
-		                      (const void*)mesh::k_mesh_colors<true>})
+		                      (const void*)mesh::k_mesh_colors<true>, (const void*)slices::k_rgba_on_grid<false>, (const void*)slices::k_rgba_on_grid<true>})
 			CU(set_smem(f, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
 		for (const void* f : {(const void*)meshopt::k_density_gradient<false, false>, (const void*)meshopt::k_density_gradient<true, false>,
 		                      (const void*)meshopt::k_density_gradient<false, true>, (const void*)meshopt::k_density_gradient<true, true>})
@@ -2078,12 +2079,7 @@ static bool grid_res_ok(const int32_t* res) {  // positive multiples of 16 (test
 	return (uint64_t)res[0] * (uint64_t)res[1] * (uint64_t)res[2] <= 0xffffffffull - 127ull;
 }
 
-extern "C" NsbStatus nsb_density_on_grid(NsbContext* c, const NsbGridQuery* q, float* density_dev, void* stream) {
-	if (!c || !q || !density_dev) return fail(NSB_ERR_INVALID, "null argument");
-	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_density_on_grid: nsb_upload_model has not been called");
-	if (!c->d_density_grid.get()) return fail(NSB_ERR_STATE, "nsb_density_on_grid: no density grid (nsb_upload_density_grid or nsb_update_density_grid)");
-	if (!grid_res_ok(q->res)) return fail(NSB_ERR_INVALID, "nsb_density_on_grid: res must be positive multiples of 16 with a 32-bit point count");
-	CU(cudaSetDevice(c->device));
+static mesh::GridQuery grid_query(const NsbGridQuery* q) {
 	mesh::GridQuery g;
 	for (int a = 0; a < 3; ++a) {
 		g.res[a] = (uint32_t)q->res[a];
@@ -2093,11 +2089,23 @@ extern "C" NsbStatus nsb_density_on_grid(NsbContext* c, const NsbGridQuery* q, f
 		g.tmin[a] = q->train_aabb_min[a];
 		g.tmax[a] = q->train_aabb_max[a];
 	}
-	const uint32_t n_padded = next_multiple_u32(g.res[0] * g.res[1] * g.res[2], 128u);
-	uint32_t grid = n_padded / 128;
+	return g;
+}
+// one 128-point tile per CTA, at most the resident CTAs of the operator-level kernels
+static uint32_t grid_ctas(const NsbContext* c, const mesh::GridQuery& g) {
+	const uint32_t grid = next_multiple_u32(g.res[0] * g.res[1] * g.res[2], 128u) / 128;
 	const uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
-	if (grid > cap) grid = cap;
-	(c->acc16 ? mesh::k_density_on_grid<true> : mesh::k_density_on_grid<false>)<<<grid, 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(
+	return grid > cap ? cap : grid;
+}
+
+extern "C" NsbStatus nsb_density_on_grid(NsbContext* c, const NsbGridQuery* q, float* density_dev, void* stream) {
+	if (!c || !q || !density_dev) return fail(NSB_ERR_INVALID, "null argument");
+	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_density_on_grid: nsb_upload_model has not been called");
+	if (!c->d_density_grid.get()) return fail(NSB_ERR_STATE, "nsb_density_on_grid: no density grid (nsb_upload_density_grid or nsb_update_density_grid)");
+	if (!grid_res_ok(q->res)) return fail(NSB_ERR_INVALID, "nsb_density_on_grid: res must be positive multiples of 16 with a 32-bit point count");
+	CU(cudaSetDevice(c->device));
+	const mesh::GridQuery g = grid_query(q);
+	(c->acc16 ? mesh::k_density_on_grid<true> : mesh::k_density_on_grid<false>)<<<grid_ctas(c, g), 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(
 		c->model, g, c->d_density_grid.get(), density_dev);
 	CU(cudaGetLastError());
 	return NSB_OK;
@@ -2290,5 +2298,85 @@ extern "C" NsbStatus nsb_mesh_optimise(NsbContext* c, const NsbMeshOptimise* p, 
 		std::swap(c->mesh_verts, c->opt_pos);  // the new positions become the mesh; the old buffer is the next step's output
 	}
 	c->mesh_normals_ok = true;
+	return NSB_OK;
+}
+
+// ---- density and RGBA slices (the export panel's "Save density PNG" / "Save RGBA PNG sequence", testbed.cu:952-966) ---------------
+static bool act_ok(int32_t a) { return a >= NSB_ACT_NONE && a <= NSB_ACT_EXPONENTIAL; }
+
+extern "C" NsbStatus nsb_rgba_on_grid(NsbContext* c, const NsbGridQuery* q, const float* ray_dir, int32_t rgb_activation, int32_t density_activation,
+                                      float* rgba_dev, void* stream) {
+	if (!c || !q || !ray_dir || !rgba_dev) return fail(NSB_ERR_INVALID, "null argument");
+	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_rgba_on_grid: nsb_upload_model has not been called");
+	if (!grid_res_ok(q->res)) return fail(NSB_ERR_INVALID, "nsb_rgba_on_grid: res must be positive multiples of 16 with a 32-bit point count");
+	if (!act_ok(rgb_activation) || !act_ok(density_activation)) return fail(NSB_ERR_INVALID, "nsb_rgba_on_grid: bad activation");
+	if ((uintptr_t)rgba_dev & 15u) return fail(NSB_ERR_INVALID, "nsb_rgba_on_grid: rgba_dev must be 16-byte aligned");
+	CU(cudaSetDevice(c->device));
+	const mesh::GridQuery g = grid_query(q);
+	(c->acc16 ? slices::k_rgba_on_grid<true> : slices::k_rgba_on_grid<false>)<<<grid_ctas(c, g), 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(
+		c->model, g, ray_dir[0], ray_dir[1], ray_dir[2], rgb_activation, density_activation, reinterpret_cast<float4*>(rgba_dev));
+	CU(cudaGetLastError());
+	return NSB_OK;
+}
+
+// the grid and its images after the optional y/z swap (marching_cubes.cu:938-945, :984-989); false unless every res is positive, the point
+// count fits 32 bits and the mosaic's width and height fit 32 bits
+static bool slices_of(const int32_t* res, int32_t swap_y_z, slices::Slices* s, uint32_t* w, uint32_t* h) {
+	if (!res || res[0] <= 0 || res[1] <= 0 || res[2] <= 0) return false;
+	if ((uint64_t)res[0] * (uint64_t)res[1] * (uint64_t)res[2] > 0xffffffffull) return false;
+	s->rx = (uint32_t)res[0]; s->ry = (uint32_t)res[1]; s->rz = (uint32_t)res[2];
+	s->swap = swap_y_z ? 1u : 0u;
+	s->sy = swap_y_z ? s->rz : s->ry;
+	s->sz = swap_y_z ? s->ry : s->rz;
+	const uint32_t ndown = (uint32_t)sqrtf((float)s->sz);
+	const uint32_t nacross = (s->sz + ndown - 1) / ndown;
+	const uint64_t ww = (uint64_t)s->rx * nacross, hh = (uint64_t)s->sy * ndown;
+	if (ww > 0xffffffffull || hh > 0xffffffffull) return false;
+	*w = (uint32_t)ww;
+	*h = (uint32_t)hh;
+	return true;
+}
+
+extern "C" NsbStatus nsb_density_png_extent(const int32_t* res, int32_t swap_y_z, uint32_t* w, uint32_t* h) {
+	if (!res || !w || !h) return fail(NSB_ERR_INVALID, "null argument");
+	slices::Slices s;
+	if (!slices_of(res, swap_y_z, &s, w, h)) return fail(NSB_ERR_INVALID, "nsb_density_png_extent: res must be positive with a 32-bit point count");
+	return NSB_OK;
+}
+
+static uint32_t slice_ctas(const NsbContext* c, uint64_t n) {
+	const uint64_t grid = (n + 255) / 256, cap = (uint64_t)c->sm_count * 8;
+	return (uint32_t)(grid < 1 ? 1 : (grid > cap ? cap : grid));
+}
+
+extern "C" NsbStatus nsb_density_png(NsbContext* c, const float* density_dev, const int32_t* res, float thresh, float density_range, int32_t swap_y_z,
+                                     uint8_t* pixels_dev, uint64_t* counts_dev, void* stream) {
+	if (!c || !density_dev || !res || !pixels_dev || !counts_dev) return fail(NSB_ERR_INVALID, "null argument");
+	slices::Slices s;
+	uint32_t w, h;
+	if (!slices_of(res, swap_y_z, &s, &w, &h)) return fail(NSB_ERR_INVALID, "nsb_density_png: res must be positive with a 32-bit point count");
+	if (!(density_range > 0.0f) || !std::isfinite(density_range)) return fail(NSB_ERR_INVALID, "nsb_density_png: density_range must be positive and finite");
+	CU(cudaSetDevice(c->device));
+	cudaStream_t st = (cudaStream_t)stream;
+	const uint32_t nacross = w / s.rx;
+	const float scale = 128.f / density_range;  // density_scale (marching_cubes.cu:899)
+	CU(cudaMemsetAsync(counts_dev, 0, 2 * sizeof(uint64_t), st));
+	const uint64_t n_px = (uint64_t)w * h;
+	slices::k_density_png<<<slice_ctas(c, n_px), 256, 0, st>>>(s, density_dev, thresh, scale, w, nacross, pixels_dev,
+	                                                            reinterpret_cast<unsigned long long*>(counts_dev));
+	CU(cudaGetLastError());
+	return NSB_OK;
+}
+
+extern "C" NsbStatus nsb_rgba_png(NsbContext* c, const float* rgba_dev, const int32_t* res, int32_t swap_y_z, uint8_t* pixels_dev, void* stream) {
+	if (!c || !rgba_dev || !res || !pixels_dev) return fail(NSB_ERR_INVALID, "null argument");
+	slices::Slices s;
+	uint32_t w, h;
+	if (!slices_of(res, swap_y_z, &s, &w, &h)) return fail(NSB_ERR_INVALID, "nsb_rgba_png: res must be positive with a 32-bit point count");
+	if (((uintptr_t)rgba_dev & 15u) || ((uintptr_t)pixels_dev & 3u)) return fail(NSB_ERR_INVALID, "nsb_rgba_png: rgba_dev must be 16-byte, pixels_dev 4-byte aligned");
+	CU(cudaSetDevice(c->device));
+	slices::k_rgba_png<<<slice_ctas(c, (uint64_t)s.rx * s.ry * s.rz), 256, 0, (cudaStream_t)stream>>>(s, reinterpret_cast<const float4*>(rgba_dev),
+	                                                                                                reinterpret_cast<uchar4*>(pixels_dev));
+	CU(cudaGetLastError());
 	return NSB_OK;
 }

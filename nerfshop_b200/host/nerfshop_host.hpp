@@ -8,6 +8,8 @@
 //                                                            compute_poisson_residual_density) once the operator is attached to a tracer
 //   ngp_b200::NerfTracer       <- Testbed::NerfTracer       (testbed.h:129-240): operator list management, trace == render
 //   ngp_b200::render_nerf(...) <- Testbed::render_nerf      (testbed.h:305, testbed_nerf.cu:3066)
+//   ngp_b200::get_rgba_on_grid, density_png, rgba_png <- Testbed::get_rgba_on_grid and the pixel loops of save_density_grid_to_png /
+//                                                       save_rgba_grid_to_png_sequence (the host keeps its own stbi_write_png)
 //
 // Errors become std::runtime_error, as CUDA_CHECK_THROW does in the reference (propagates to main.cu:252).
 #pragma once
@@ -19,6 +21,14 @@
 #include <vector>
 
 #include "../../include/nerfshop_b200.h"
+
+// density_png / rgba_png hand host pixels back and need the CUDA runtime for their device scratch; the rest of the shim does not
+#if defined(__has_include)
+#if __has_include(<cuda_runtime_api.h>)
+#include <cuda_runtime_api.h>
+#define NSB_HOST_HAVE_CUDART 1
+#endif
+#endif
 
 namespace ngp_b200 {
 
@@ -183,5 +193,69 @@ inline Mesh marching_cubes(Context& ctx, NsbGridQuery q, float* density_dev, flo
 inline void optimise_mesh_step(Context& ctx, const NsbMeshOptimise& p, uint32_t n_steps, void* stream) {
 	check(nsb_mesh_optimise(ctx.get(), &p, n_steps, stream), "nsb_mesh_optimise");
 }
+
+// Testbed::get_rgba_on_grid (testbed_nerf.cu:4588-4612): premultiplied RGBA of the field seen from ray_dir at the grid points of q (the
+// reference samples m_render_aabb; q.res as the reference passes it, multiples of 16) into caller device memory (float4 per point).
+inline void get_rgba_on_grid(Context& ctx, const NsbGridQuery& q, const float ray_dir[3], int32_t rgb_activation, int32_t density_activation, float* rgba_dev,
+                             void* stream) {
+	check(nsb_rgba_on_grid(ctx.get(), &q, ray_dir, rgb_activation, density_activation, rgba_dev, stream), "nsb_rgba_on_grid");
+}
+
+#ifdef NSB_HOST_HAVE_CUDART
+namespace detail {
+struct CudaFree { void operator()(void* p) const { cudaFree(p); } };
+inline std::unique_ptr<void, CudaFree> device_alloc(size_t bytes) {
+	void* p = nullptr;
+	if (cudaMalloc(&p, bytes) != cudaSuccess) throw std::runtime_error("cudaMalloc failed");
+	return std::unique_ptr<void, CudaFree>(p);
+}
+inline void download(void* dst, const void* src, size_t bytes, void* stream) {
+	if (cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, (cudaStream_t)stream) != cudaSuccess || cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess)
+		throw std::runtime_error("device-to-host copy failed");
+}
+}  // namespace detail
+
+// save_density_grid_to_png (marching_cubes.cu:898-974) up to its stbi_write_png(filename, w, h, 1, pixels.data(), w) and its log line,
+// for a device float grid such as Testbed::get_density_on_grid's (compute_and_save_png_slices, testbed.cu:345-366).
+struct DensityPng {
+	uint32_t w = 0, h = 0;
+	std::vector<uint8_t> pixels;  // w * h
+	uint64_t n_zero_x_voxels = 0, n_lattice_near_zero_x = 0;
+};
+inline DensityPng density_png(Context& ctx, const float* density_dev, const int32_t res[3], float thresh, float density_range, bool swap_y_z, void* stream) {
+	DensityPng p;
+	check(nsb_density_png_extent(res, swap_y_z ? 1 : 0, &p.w, &p.h), "nsb_density_png_extent");
+	p.pixels.resize((size_t)p.w * p.h);
+	const size_t counts_at = (p.pixels.size() + 7) & ~size_t(7);  // the counts after the pixels, 8-byte aligned
+	auto px = detail::device_alloc(counts_at + 2 * sizeof(uint64_t));
+	uint64_t* counts = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(px.get()) + counts_at);
+	check(nsb_density_png(ctx.get(), density_dev, res, thresh, density_range, swap_y_z ? 1 : 0, static_cast<uint8_t*>(px.get()), counts, stream), "nsb_density_png");
+	uint64_t c[2];
+	detail::download(p.pixels.data(), px.get(), p.pixels.size(), stream);
+	detail::download(c, counts, sizeof(c), stream);
+	p.n_zero_x_voxels = c[0];
+	p.n_lattice_near_zero_x = c[1];
+	return p;
+}
+
+// save_rgba_grid_to_png_sequence (marching_cubes.cu:979-1015) up to its stbi_write_png(path/%04d_<w>x<h>.png, w, h, 4, slice z, w * 4),
+// for a device float4 grid such as get_rgba_on_grid's.
+struct RgbaPng {
+	uint32_t w = 0, h = 0, n_slices = 0;
+	std::vector<uint8_t> pixels;  // n_slices images of w * h * 4 bytes, back to back
+	const uint8_t* slice(uint32_t z) const { return pixels.data() + (size_t)z * w * h * 4; }
+};
+inline RgbaPng rgba_png(Context& ctx, const float* rgba_dev, const int32_t res[3], bool swap_y_z, void* stream) {
+	RgbaPng p;
+	p.w = (uint32_t)res[0];
+	p.h = (uint32_t)(swap_y_z ? res[2] : res[1]);
+	p.n_slices = (uint32_t)(swap_y_z ? res[1] : res[2]);
+	p.pixels.resize((size_t)p.w * p.h * p.n_slices * 4);
+	auto px = detail::device_alloc(p.pixels.size());
+	check(nsb_rgba_png(ctx.get(), rgba_dev, res, swap_y_z ? 1 : 0, static_cast<uint8_t*>(px.get()), stream), "nsb_rgba_png");
+	detail::download(p.pixels.data(), px.get(), p.pixels.size(), stream);
+	return p;
+}
+#endif  // NSB_HOST_HAVE_CUDART
 
 }  // namespace ngp_b200

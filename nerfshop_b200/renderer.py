@@ -7,6 +7,8 @@
   NerfRenderer.{add,reset}_edit_operator <- NerfTracer::{add,reset}_edit_operator (testbed.h:129-240)
   NerfRenderer.density_on_grid / marching_cubes / mesh_shade / mesh_download <- Testbed::marching_cubes (testbed_nerf.cu:4614-4649);
       nerfshop_b200.mesh builds the reference's Python-facing calls on them
+  NerfRenderer.rgba_on_grid / density_png / rgba_png <- Testbed::get_rgba_on_grid (testbed_nerf.cu:4588-4612) and the pixel loops of
+      save_density_grid_to_png / save_rgba_grid_to_png_sequence (marching_cubes.cu:898-1015); nerfshop_b200.slices writes the files
 
 torch is used for device memory and streams only; every computation is a call into libnerfshop_b200.so.
 """
@@ -16,7 +18,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import abi
+from . import abi, slices
 
 
 def _torch():
@@ -385,3 +387,48 @@ class NerfRenderer:
         abi.check(self.lib, self.lib.nsb_mesh_download(self.ctx, V.ctypes.data, None if N is None else N.ctypes.data, None if Cc is None else Cc.ctypes.data,
                                                        rows, F.ctypes.data, F.size), "nsb_mesh_download")
         return dict(V=V, N=N, C=Cc, F=F)
+
+    # ---- density and RGBA slices (the export panel, testbed.cu:952-966) -----------------------------------------------------------
+    def rgba_on_grid(self, res3d, aabb, train_aabb, ray_dir, rgb_activation: int = abi.NSB_ACT_LOGISTIC,
+                     density_activation: int = abi.NSB_ACT_EXPONENTIAL, out=None, stream=None):
+        """Testbed::get_rgba_on_grid: float32 CUDA tensor [res_z, res_y, res_x, 4] (x fastest) of compute_nerf_density's premultiplied
+        rgb and alpha, the network seen from ray_dir at the grid positions of density_on_grid over aabb. res3d: positive multiples of 16."""
+        torch = _torch()
+        q = abi.NsbGridQuery()
+        q.res[:] = [int(v) for v in res3d]
+        q.aabb_min[:], q.aabb_max[:] = [float(v) for v in aabb[0]], [float(v) for v in aabb[1]]
+        q.train_aabb_min[:], q.train_aabb_max[:] = [float(v) for v in train_aabb[0]], [float(v) for v in train_aabb[1]]
+        d = (C.c_float * 3)(*[float(v) for v in ray_dir])
+        if out is None:
+            out = torch.empty((max(q.res[2], 0), max(q.res[1], 0), max(q.res[0], 0), 4), dtype=torch.float32, device=torch.device("cuda", self.device))
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_rgba_on_grid(self.ctx, C.byref(q), d, int(rgb_activation), int(density_activation), out.data_ptr(), s),
+                  "nsb_rgba_on_grid")
+        return out
+
+    def density_png(self, density, res3d, thresh: float, density_range: float = 4.0, swap_y_z: bool = False, stream=None):
+        """save_density_grid_to_png's pixels and counts on a float32 CUDA grid of res3d points (x fastest): (uint8 CUDA tensor [h, w], the
+        mosaic of the z slices; int64 CUDA tensor [2]: #zero-x voxels, #lattice near zero-x)."""
+        torch = _torch()
+        w, h = slices.density_png_extent(res3d, swap_y_z)
+        res = (C.c_int32 * 3)(*[int(v) for v in res3d])
+        dev = torch.device("cuda", self.device)
+        pixels = torch.empty((h, w), dtype=torch.uint8, device=dev)
+        counts = torch.empty(2, dtype=torch.int64, device=dev)
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_density_png(self.ctx, density.data_ptr(), res, float(thresh), float(density_range), int(bool(swap_y_z)),
+                                                     pixels.data_ptr(), counts.data_ptr(), s), "nsb_density_png")
+        return pixels, counts
+
+    def rgba_png(self, rgba, res3d, swap_y_z: bool = False, stream=None):
+        """save_rgba_grid_to_png_sequence's pixels on a float32 CUDA tensor of res3d RGBA points (x fastest): uint8 CUDA tensor
+        [slices, h, w, 4], slice z being the image of file %04d_<w>x<h>.png (with the swap: res_y slices of res_z rows)."""
+        torch = _torch()
+        rx, ry, rz = [int(v) for v in res3d]
+        h, n = (rz, ry) if swap_y_z else (ry, rz)
+        res = (C.c_int32 * 3)(rx, ry, rz)
+        pixels = torch.empty((max(n, 0), max(h, 0), max(rx, 0), 4), dtype=torch.uint8, device=torch.device("cuda", self.device))
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_rgba_png(self.ctx, rgba.data_ptr(), res, int(bool(swap_y_z)), pixels.data_ptr(), s), "nsb_rgba_png")
+        return pixels
+
