@@ -319,7 +319,10 @@ typedef struct {
  * (EditOperator::map_positions, :3593-3599), evaluates NerfNetwork::density, activates, adds the membrane residual densities
  * (compute_poisson_residual_density, cage_deformation.cu:341-383), max-splats into a scratch grid (:447-463), merges into the
  * context's running density grid (ema_grid_samples_nerf, :483-506) and rebuilds the occupancy bitfield the renderer marches.
- * The running grid is the one nsb_upload_density_grid stored (all zeros if none was uploaded). Stream-ordered. */
+ * The running grid is the one nsb_upload_density_grid stored (all zeros if none was uploaded). Stream-ordered.
+ * NSB_ERR_INVALID, before anything is launched, if n_uniform_samples + n_nonuniform_samples exceeds NSB_GRID_UPDATE_MAX_SAMPLES
+ * (2^31, over 200 times the reference's largest update, 5 x 128^3). */
+#define NSB_GRID_UPDATE_MAX_SAMPLES (1ull << 31)
 NsbStatus nsb_update_density_grid(NsbContext* ctx, const NsbGridUpdate* params, void* stream);
 /* copies the context's running density grid (HOST float[5*128^3], may be NULL) and occupancy bitfield (HOST, NSB_BITFIELD_BYTES,
  * may be NULL) back; synchronises the device. */

@@ -17,6 +17,7 @@ NSB_NERF_GRIDSIZE = 128
 NSB_NERF_CASCADES = 5
 NSB_GRID_CELLS = NSB_NERF_CASCADES * NSB_NERF_GRIDSIZE ** 3
 NSB_BITFIELD_BYTES = NSB_GRID_CELLS // 8
+NSB_GRID_UPDATE_MAX_SAMPLES = 1 << 31
 
 NSB_OK, NSB_ERR_INVALID, NSB_ERR_CUDA, NSB_ERR_STATE, NSB_ERR_UNSUPPORTED = range(5)
 

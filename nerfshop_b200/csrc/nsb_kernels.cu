@@ -748,7 +748,8 @@ __global__ void __launch_bounds__(128) k_density_grid_update(const DevModel m, c
 			// Work assignment (not semantics): the reference's thread li draws cell (li*A + B) mod 128^3, a pseudo-random permutation,
 			// so a warp's 32 samples scatter over the whole volume. Every sample is independent and the splat is an order-free max, so
 			// thread t instead takes the sample whose first-choice cell is t mod 128^3: a warp covers a 4x4x2 Morton block of cells and
-			// its hash-grid gathers share sectors (53369 = 56924617^-1 mod 2^21). Exact for whole multiples of 128^3 samples (the reference's post-edit setting).
+			// its hash-grid gathers share sectors (53369 = 56924617^-1 mod 2^21). Only whole 128^3 blocks of a launch are permuted, each within
+			// itself, and a ragged tail keeps the reference's assignment, so every launch draws the reference's set of samples at any count.
 			if (li < (n_el & ~(GRIDVOL - 1u)))
 				li = (li & ~(GRIDVOL - 1u)) | ((((li & (GRIDVOL - 1u)) - 96925573u) * 53369u - a.step * n_el) & (GRIDVOL - 1u));
 			Pcg32 rng;
@@ -1278,7 +1279,8 @@ extern "C" NsbStatus nsb_update_density_grid(NsbContext* c, const NsbGridUpdate*
 	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_upload_model has not been called");
 	if (u->n_cascades < 1 || u->n_cascades > NSB_NERF_CASCADES) return fail(NSB_ERR_INVALID, "n_cascades must be in [1, 5]");
 	const uint64_t n_total64 = (uint64_t)u->n_uniform_samples + u->n_nonuniform_samples;
-	if (n_total64 > 0xffffff00ull) return fail(NSB_ERR_INVALID, "too many grid samples");
+	// k_density_grid_update's 32-bit grid-stride index must not wrap: base < 2^31 plus one stride of at most a few thousand CTAs x 128
+	if (n_total64 > NSB_GRID_UPDATE_MAX_SAMPLES) return fail(NSB_ERR_INVALID, "n_uniform_samples + n_nonuniform_samples exceeds 2^31");
 	CU(cudaSetDevice(c->device));
 	cudaStream_t st = (cudaStream_t)stream_;
 	NsbStatus rc = ensure_grid_buffers(c);

@@ -1317,8 +1317,11 @@ void orc_pcg32_advance(uint64_t* state_inc, uint64_t delta) {
 
 // Testbed::update_density_grid_nerf_operator (testbed_nerf.cu:3533-3639) on the host; `grid` is the running density grid
 // (in/out, 5*128^3), `bits` receives update_density_grid_mean_and_bitfield's result. `samples_out` (optional, n x 4 floats)
-// receives {mapped warped position, activated+residual density} per sample for diagnostics.
-int orc_update_density_grid(const OrcScene* s, const NsbGridUpdate* u, float* grid, uint8_t* bits, float* mean_out, float* samples_out) {
+// receives {mapped warped position, activated+residual density} per sample for diagnostics. `cells_out` (optional, n uint32) receives
+// each sample's splat cell (cascade * 128^3 + Morton index) and `residual_out` (optional, n fp16 bits) the membrane residual half
+// added to its activated density: 0 if none was added, NaN (0x7e00) if more than one operator added one.
+int orc_update_density_grid(const OrcScene* s, const NsbGridUpdate* u, float* grid, uint8_t* bits, float* mean_out, float* samples_out,
+                            uint32_t* cells_out, uint16_t* residual_out) {
 	Model m;
 	if (!model_init(m, &s->desc, s->params, s->n_params)) return 1;
 	const uint32_t n_cells = GRIDVOL * (uint32_t)CASCADES;
@@ -1359,6 +1362,8 @@ int orc_update_density_grid(const OrcScene* s, const NsbGridUpdate* u, float* gr
 		uint16_t o[16], d16[16];
 		network_forward(m, pw, v3(0.5f, 0.5f, 0.5f), o, d16, true);                             // NerfNetwork::density (:3601-3603)
 		uint16_t h = f2h(network_to_density(h2f(d16[0]), u->density_activation));               // activate_network_density (:3522-3531)
+		uint16_t residual = 0;
+		int n_residuals = 0;
 		if (u->apply_operators) {
 			for (int k = s->n_ops - 1; k >= 0; --k) {                                           // compute_poisson_residual_density (:3612-3620)
 				const NsbEditOp& op = s->ops[k];
@@ -1373,7 +1378,9 @@ int orc_update_density_grid(const OrcScene* s, const NsbGridUpdate* u, float* gr
 				const uint32_t* tv = op.tets + 4 * (size_t)t;
 				float res = fmaf(b[3], op.boundary_residual_density[tv[3]], fmaf(b[2], op.boundary_residual_density[tv[2]],
 				            fmaf(b[0], op.boundary_residual_density[tv[0]], b[1] * op.boundary_residual_density[tv[1]])));
-				h = hadd(h, f2h(res));                                                          // half += half (:379)
+				residual = f2h(res);
+				++n_residuals;
+				h = hadd(h, residual);                                                          // half += half (:379)
 			}
 		}
 		const float ot = h2f(h) * MIN_STEP();                                                   // splat_..._already_activated (:447-463)
@@ -1383,6 +1390,8 @@ int orc_update_density_grid(const OrcScene* s, const NsbGridUpdate* u, float* gr
 		uint32_t cur = __atomic_load_n(cell, __ATOMIC_RELAXED);
 		while (ob > cur && !__atomic_compare_exchange_n(cell, &cur, ob, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
 		if (samples_out) { samples_out[4 * (size_t)i] = pw.x; samples_out[4 * (size_t)i + 1] = pw.y; samples_out[4 * (size_t)i + 2] = pw.z; samples_out[4 * (size_t)i + 3] = h2f(h); }
+		if (cells_out) cells_out[i] = idx;
+		if (residual_out) residual_out[i] = n_residuals > 1 ? (uint16_t)0x7e00u : residual;
 	}
 	for (uint32_t i = 0; i < n_cells; ++i) {                                                   // ema_grid_samples_nerf (:483-506)
 		float imp;

@@ -78,7 +78,8 @@ def lib() -> C.CDLL:
         l.orc_pcg32_next.restype = None
         l.orc_pcg32_advance.argtypes = [C.c_void_p, C.c_uint64]
         l.orc_pcg32_advance.restype = None
-        l.orc_update_density_grid.argtypes = [C.POINTER(OrcScene), C.POINTER(abi.NsbGridUpdate), C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.c_void_p]
+        l.orc_update_density_grid.argtypes = [C.POINTER(OrcScene), C.POINTER(abi.NsbGridUpdate), C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.c_void_p,
+                                              C.c_void_p, C.c_void_p]
         l.orc_poisson_boundary.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_uint32, C.POINTER(abi.NsbBoundarySampling), C.c_void_p, C.c_void_p, C.c_void_p]
         l.orc_poisson_boundary_ex.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_uint32, C.POINTER(abi.NsbBoundarySampling), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         l.orc_membrane_blend.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32] + [C.c_void_p] * 7
@@ -156,16 +157,21 @@ class Oracle:
         assert self.lib.orc_march_trace(C.byref(self.scene), C.byref(frame), _ptr(pixels), n, max_samples, _ptr(rec), _ptr(idx), _ptr(cnt)) == 0
         return rec, idx, cnt
 
-    def update_density_grid(self, params: "abi.NsbGridUpdate", grid: np.ndarray, want_samples: bool = False):
-        """Testbed::update_density_grid_nerf_operator on the host. Returns (grid, bitfield, mean[, samples])."""
+    def update_density_grid(self, params: "abi.NsbGridUpdate", grid: np.ndarray, want_samples: bool = False, want_splats: bool = False):
+        """Testbed::update_density_grid_nerf_operator on the host. Returns (grid, bitfield, mean[, samples][, splats]).
+        samples: float32 [n, 4] {mapped warped position, activated + residual density}. splats: (cell uint32 [n], the sample's splat
+        cell; residual uint16 [n], the fp16 bits of the membrane residual added to its activated density: 0 if none, NaN if several)."""
         grid = np.ascontiguousarray(grid, np.float32).reshape(-1).copy()
         bits = np.zeros(abi.NSB_BITFIELD_BYTES, np.uint8)
         mean = C.c_float()
         n = params.n_uniform_samples + params.n_nonuniform_samples
         samples = np.zeros((n, 4), np.float32) if want_samples else None
-        rc = self.lib.orc_update_density_grid(C.byref(self.scene), C.byref(params), _ptr(grid), _ptr(bits), C.byref(mean), None if samples is None else _ptr(samples))
+        cells = np.zeros(n, np.uint32) if want_splats else None
+        residual = np.zeros(n, np.uint16) if want_splats else None
+        rc = self.lib.orc_update_density_grid(C.byref(self.scene), C.byref(params), _ptr(grid), _ptr(bits), C.byref(mean),
+                                              *[None if a is None else _ptr(a) for a in (samples, cells, residual)])
         assert rc == 0
-        return (grid, bits, mean.value, samples) if want_samples else (grid, bits, mean.value)
+        return (grid, bits, mean.value) + ((samples,) if want_samples else ()) + (((cells, residual),) if want_splats else ())
 
     def poisson_boundary_with_jitter(self, points: np.ndarray, params: "abi.NsbBoundarySampling", uniforms: np.ndarray):
         """compute_poisson_boundary with the jitter given (2 uniforms per sample, (vertex, i, j) order) instead of drawn from pcg32: (density, shs, coords)."""
