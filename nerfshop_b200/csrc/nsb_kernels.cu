@@ -152,6 +152,29 @@ __device__ __forceinline__ void encode_to_a32(uint8_t* a32, const DevModel& m, b
 	}
 }
 
+// The loop of the one-tile network kernels (one CTA = 128 threads = one tile of 128 rows, tc::TileSmem of dynamic shared memory,
+// grid-stride over the n_padded rows). sample(i, pw, dw) runs for valid rows (i < n) only and sets the row's warped position and
+// direction; the other rows keep the origin and dw_default. emit(i, valid, pw, dens, rgbo) runs for every row i < n_padded, the
+// padding included, with the network's outputs (density_only: the density MLP alone). n_padded must be a multiple of 128: emit is
+// called for every row of every tile, so a partial last tile would reach past n_padded.
+template <bool ACC16, typename Sample, typename Emit>
+__device__ __forceinline__ void network_tiles(const DevModel& m, uint32_t n, uint32_t n_padded, bool density_only, V3 dw_default, Sample sample, Emit emit) {
+	extern __shared__ __align__(128) uint8_t smem_raw[];
+	tc::TileSmem& S = *reinterpret_cast<tc::TileSmem*>(smem_raw);
+	const uint32_t tid = threadIdx.x;
+	tc::tile_setup(S, m.w_image);
+	for (uint32_t base = blockIdx.x * 128u; base < n_padded; base += gridDim.x * 128u) {
+		const uint32_t i = base + tid;
+		const bool valid = i < n;
+		V3 pw = v3(0, 0, 0), dw = dw_default;
+		if (valid) sample(i, pw, dw);
+		uint32_t dens[8], rgbo[8];
+		encode_to_a32(S.a32, m, valid, pw, tid);
+		tc::run_network<ACC16>(tc::single_tile_ctx(S), dw, density_only, dens, rgbo);
+		emit(i, valid, pw, dens, rgbo);
+	}
+}
+
 __device__ __forceinline__ float h_lo(uint32_t packed) { return __half2float(__ushort_as_half((unsigned short)(packed & 0xffffu))); }
 __device__ __forceinline__ float h_hi(uint32_t packed) { return __half2float(__ushort_as_half((unsigned short)(packed >> 16))); }
 
@@ -521,31 +544,18 @@ __global__ void __launch_bounds__(128 * render_tiles(OPS, ACC16), 1) k_render_fu
 template <bool DENSITY_ONLY, bool ACC16>
 __global__ void __launch_bounds__(128) k_inference(const DevModel m, const float* __restrict__ coords, uint32_t n, __half* __restrict__ out,
                                                    uint32_t n_padded) {
-	extern __shared__ __align__(128) uint8_t smem_raw[];
-	tc::TileSmem& S = *reinterpret_cast<tc::TileSmem*>(smem_raw);
-	const uint32_t tid = threadIdx.x;
-	tc::tile_setup(S, m.w_image);
-	for (uint32_t base = blockIdx.x * 128u; base < n_padded; base += gridDim.x * 128u) {
-		uint32_t i = base + tid;
-		bool valid = i < n;
-		V3 pw = v3(0, 0, 0), dw = v3(0.5f, 0.5f, 0.5f);
-		if (valid) {
-			pw = v3(coords[7 * (size_t)i], coords[7 * (size_t)i + 1], coords[7 * (size_t)i + 2]);
-			dw = v3(coords[7 * (size_t)i + 4], coords[7 * (size_t)i + 5], coords[7 * (size_t)i + 6]);
-		}
-		uint32_t dens[8], rgbo[8];
-		encode_to_a32(S.a32, m, valid, pw, tid);
-		tc::run_network<ACC16>(tc::single_tile_ctx(S), dw, DENSITY_ONLY, dens, rgbo);
-		if (i < n_padded) {
-			const uint32_t* src = DENSITY_ONLY ? dens : rgbo;
+	network_tiles<ACC16>(m, n, n_padded, DENSITY_ONLY, v3(0.5f, 0.5f, 0.5f), [&](uint32_t i, V3& pw, V3& dw) {
+		pw = v3(coords[7 * (size_t)i], coords[7 * (size_t)i + 1], coords[7 * (size_t)i + 2]);
+		dw = v3(coords[7 * (size_t)i + 4], coords[7 * (size_t)i + 5], coords[7 * (size_t)i + 6]);
+	}, [&](uint32_t i, bool, V3, const uint32_t* dens, const uint32_t* rgbo) {  // every row: the padding gets the output of the zero input
+		const uint32_t* src = DENSITY_ONLY ? dens : rgbo;
 #pragma unroll
-			for (int k = 0; k < 8; ++k) {
-				out[(size_t)(2 * k) * n_padded + i] = __ushort_as_half((unsigned short)(src[k] & 0xffffu));
-				out[(size_t)(2 * k + 1) * n_padded + i] = __ushort_as_half((unsigned short)(src[k] >> 16));
-			}
-			if (!DENSITY_ONLY) out[(size_t)3 * n_padded + i] = __ushort_as_half((unsigned short)(dens[0] & 0xffffu));  // extract_density
+		for (int k = 0; k < 8; ++k) {
+			out[(size_t)(2 * k) * n_padded + i] = __ushort_as_half((unsigned short)(src[k] & 0xffffu));
+			out[(size_t)(2 * k + 1) * n_padded + i] = __ushort_as_half((unsigned short)(src[k] >> 16));
 		}
-	}
+		if (!DENSITY_ONLY) out[(size_t)3 * n_padded + i] = __ushort_as_half((unsigned short)(dens[0] & 0xffffu));  // extract_density
+	});
 }
 
 // tcnn GridEncoding inference alone: fp16 [32 x n_padded] row-major, same loop body as the fused kernel.
@@ -633,13 +643,9 @@ __global__ void k_map_positions(const DevOp* __restrict__ ops, int n_ops, float*
 	if (empty && empty_mask) empty_mask[i] = 1;
 }
 
-// EditOperator::compute_poisson_residual_density (compute_poisson_residual_density_kernel, cage_deformation.cu:341-383):
-// density_network_output[i] += (half) interpolated residual density, for the first tet that contains the (warped) position
-__global__ void k_poisson_residual_density(const DevOp* __restrict__ ops, int n_ops, const float* __restrict__ pos, uint32_t stride, __half* __restrict__ density_out, uint32_t n) {
-	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
-	const float* q = pos + (size_t)i * stride;
-	const V3 pw = v3(q[0], q[1], q[2]);
+// The loop of compute_poisson_residual_density_kernel (cage_deformation.cu:341-383): h += (half) interpolated residual density, for the
+// first tet that contains the (warped) position pw, of each operator in reverse order
+__device__ __forceinline__ void add_residual_density(const DevOp* __restrict__ ops, int n_ops, V3 pw, __half& h) {
 	for (int o = n_ops - 1; o >= 0; --o) {
 		const DevOp& op = ops[o];
 		if (op.type != 0 || !op.apply_poisson || !op.has_poisson_data || op.n_tets == 0) continue;
@@ -650,8 +656,16 @@ __global__ void k_poisson_residual_density(const DevOp* __restrict__ ops, int n_
 		if (t < 0) continue;
 		uint4 tv = __ldg(reinterpret_cast<const uint4*>(op.tets) + t);
 		float res = bary_mix1(b, __ldg(op.rd + tv.x), __ldg(op.rd + tv.y), __ldg(op.rd + tv.z), __ldg(op.rd + tv.w));
-		density_out[i] = __hadd(density_out[i], __float2half_rn(res));
+		h = __hadd(h, __float2half_rn(res));
 	}
+}
+
+// EditOperator::compute_poisson_residual_density: density_network_output[i] += the residual densities at position i
+__global__ void k_poisson_residual_density(const DevOp* __restrict__ ops, int n_ops, const float* __restrict__ pos, uint32_t stride, __half* __restrict__ density_out, uint32_t n) {
+	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const float* q = pos + (size_t)i * stride;
+	add_residual_density(ops, n_ops, v3(q[0], q[1], q[2]), density_out[i]);
 }
 
 template <bool GENERAL>
@@ -720,6 +734,8 @@ __global__ void k_bitfield_max_pool(uint32_t n, const uint8_t* __restrict__ prev
 // -> hash encode + density MLP on wgmma (NerfNetwork::density) -> activate (:3522-3531) -> membrane residual density
 // (cage_deformation.cu:341-383) -> max-splat (:447-463). The reference materialises positions, indices, a bool mask and the
 // 16 x N fp16 density matrix between seven launches; here a sample lives in registers and shared memory from draw to splat.
+// It keeps its own copy of network_tiles' loop: written on network_tiles, the same code compiles to a longer hash-grid gather loop
+// and runs slower.
 struct GridUpdateArgs {
 	uint32_t n_uniform, n_total, n_cascades, step;
 	uint64_t rng_state, rng_inc;
@@ -780,20 +796,7 @@ __global__ void __launch_bounds__(128) k_density_grid_update(const DevModel m, c
 		tc::run_network<ACC16>(tc::single_tile_ctx(S), dw, true, dens, rgbo);
 		if (valid) {
 			__half h = __float2half_rn(network_to_density(__half2float(__ushort_as_half((unsigned short)(dens[0] & 0xffffu))), a.density_activation));
-			if (a.apply_ops) {
-				for (int o = n_ops - 1; o >= 0; --o) {  // :3612-3620; looked up at the MAPPED position, as the reference does
-					const DevOp& op = ops[o];
-					if (op.type != 0 || !op.apply_poisson || !op.has_poisson_data || op.n_tets == 0) continue;
-					V3 p = unwarp_position(pw, op.amin, op.amax);
-					if (!box_contains(op.bmin, op.bmax, p)) continue;
-					float b[4];
-					int t = find_tet(op, p, b);
-					if (t < 0) continue;
-					uint4 tv = __ldg(reinterpret_cast<const uint4*>(op.tets) + t);
-					float res = bary_mix1(b, __ldg(op.rd + tv.x), __ldg(op.rd + tv.y), __ldg(op.rd + tv.z), __ldg(op.rd + tv.w));
-					h = __hadd(h, __float2half_rn(res));
-				}
-			}
+			if (a.apply_ops) add_residual_density(ops, n_ops, pw, h);  // :3612-3620; looked up at the MAPPED position, as the reference does
 			const float optical_thickness = mul(__half2float(h), MIN_STEP());
 			atomicMax(reinterpret_cast<unsigned int*>(grid_tmp) + idx, __float_as_uint(optical_thickness));  // uint order == float order for >= 0
 		}
@@ -1051,6 +1054,13 @@ struct NsbContext {
 
 static uint32_t next_multiple_u32(uint32_t v, uint32_t m) { return ((v + m - 1) / m) * m; }
 
+// The grid of a one-tile kernel over n_rows rows: one 128-row tile per CTA, at most ctas_per_sm resident CTAs per SM (the kernels
+// stride over the rest)
+static uint32_t tile_ctas(const NsbContext* c, uint64_t n_rows, int ctas_per_sm) {
+	const uint64_t tiles = (n_rows + 127) / 128, cap = (uint64_t)c->sm_count * ctas_per_sm;
+	return (uint32_t)(tiles < cap ? tiles : cap);
+}
+
 static const uint64_t kMlpParams = 64 * 32 + 16 * 64 + 64 * 32 + 64 * 64 + 16 * 64;
 
 extern "C" int nsb_abi_version(void) { return NSB_ABI_VERSION; }
@@ -1111,32 +1121,29 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 	CU(set_smem((const void*)k_render_fused<true, true, false>, sizeof(RenderSmemT<render_tiles(true, true)>), 1));
 	cudaFuncAttributes fa;
 	CU(cudaFuncGetAttributes(&fa, k_render_fused<false, true, true>));
-	const int by_smem_tile = (int)(prop.sharedMemPerMultiprocessor / (sizeof(tc::TileSmem) + 1024));
-	{   // the operator-level kernels: one tile per CTA, residency from registers / shared memory
+	// the operator-level kernels: one tile per CTA, residency from registers / shared memory, 1 to 5 CTAs per SM
+	auto tile_ctas_per_sm = [&](const void* func, int* ctas) -> cudaError_t {
 		cudaFuncAttributes fi;
-		CU(cudaFuncGetAttributes(&fi, k_inference<false, false>));
-		int r = fi.numRegs > 0 ? (int)(prop.regsPerMultiprocessor / (fi.numRegs * 128)) : 4;
-		c->inference_ctas_per_sm = r < by_smem_tile ? r : by_smem_tile;
-		if (c->inference_ctas_per_sm > 5) c->inference_ctas_per_sm = 5;
-		if (c->inference_ctas_per_sm < 1) c->inference_ctas_per_sm = 1;
-		CU(cudaFuncGetAttributes(&fi, k_density_grid_update<false>));
-		r = fi.numRegs > 0 ? (int)(prop.regsPerMultiprocessor / (fi.numRegs * 128)) : 4;
-		c->grid_update_ctas_per_sm = r < by_smem_tile ? r : by_smem_tile;
-		if (c->grid_update_ctas_per_sm > 5) c->grid_update_ctas_per_sm = 5;
-		if (c->grid_update_ctas_per_sm < 1) c->grid_update_ctas_per_sm = 1;
-		CU(set_smem((const void*)k_inference<false, false>, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
-		CU(set_smem((const void*)k_inference<true, false>, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
-		CU(set_smem((const void*)k_inference<false, true>, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
-		CU(set_smem((const void*)k_inference<true, true>, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
-		CU(set_smem((const void*)k_density_grid_update<false>, sizeof(tc::TileSmem), c->grid_update_ctas_per_sm));
-		CU(set_smem((const void*)k_density_grid_update<true>, sizeof(tc::TileSmem), c->grid_update_ctas_per_sm));
-		for (const void* f : {(const void*)mesh::k_density_on_grid<false>, (const void*)mesh::k_density_on_grid<true>, (const void*)mesh::k_mesh_colors<false>,
-		                      (const void*)mesh::k_mesh_colors<true>, (const void*)slices::k_rgba_on_grid<false>, (const void*)slices::k_rgba_on_grid<true>})
-			CU(set_smem(f, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
-		for (const void* f : {(const void*)meshopt::k_density_gradient<false, false>, (const void*)meshopt::k_density_gradient<true, false>,
-		                      (const void*)meshopt::k_density_gradient<false, true>, (const void*)meshopt::k_density_gradient<true, true>})
-			CU(set_smem(f, sizeof(meshopt::GradSmem), c->inference_ctas_per_sm));
-	}
+		const cudaError_t e = cudaFuncGetAttributes(&fi, func);
+		if (e != cudaSuccess) return e;
+		const int by_regs = fi.numRegs > 0 ? (int)(prop.regsPerMultiprocessor / (fi.numRegs * 128)) : 4;
+		const int by_smem = (int)(prop.sharedMemPerMultiprocessor / (sizeof(tc::TileSmem) + 1024));
+		const int r = by_regs < by_smem ? by_regs : by_smem;
+		*ctas = r > 5 ? 5 : r < 1 ? 1 : r;
+		return cudaSuccess;
+	};
+	CU(tile_ctas_per_sm((const void*)k_inference<false, false>, &c->inference_ctas_per_sm));
+	CU(tile_ctas_per_sm((const void*)k_density_grid_update<false>, &c->grid_update_ctas_per_sm));
+	for (const void* f : {(const void*)k_inference<false, false>, (const void*)k_inference<true, false>, (const void*)k_inference<false, true>,
+	                      (const void*)k_inference<true, true>, (const void*)mesh::k_density_on_grid<false>, (const void*)mesh::k_density_on_grid<true>,
+	                      (const void*)mesh::k_mesh_colors<false>, (const void*)mesh::k_mesh_colors<true>, (const void*)slices::k_rgba_on_grid<false>,
+	                      (const void*)slices::k_rgba_on_grid<true>})
+		CU(set_smem(f, sizeof(tc::TileSmem), c->inference_ctas_per_sm));
+	for (const void* f : {(const void*)k_density_grid_update<false>, (const void*)k_density_grid_update<true>})
+		CU(set_smem(f, sizeof(tc::TileSmem), c->grid_update_ctas_per_sm));
+	for (const void* f : {(const void*)meshopt::k_density_gradient<false, false>, (const void*)meshopt::k_density_gradient<true, false>,
+	                      (const void*)meshopt::k_density_gradient<false, true>, (const void*)meshopt::k_density_gradient<true, true>})
+		CU(set_smem(f, sizeof(meshopt::GradSmem), c->inference_ctas_per_sm));
 	if (getenv("NSB_VERBOSE"))
 		fprintf(stderr, "[nsb] device %d: %d SMs; k_render_fused %d tiles/CTA (%d with fp32 accumulators, %d with operators), %d regs, %zu B smem; inference %d CTAs/SM, grid update %d CTAs/SM\n",
 		        device, c->sm_count, render_tiles(false, true), render_tiles(false, false), render_tiles(true, true), fa.numRegs, sizeof(RenderSmemT<render_tiles(false, true)>),
@@ -1295,10 +1302,7 @@ extern "C" NsbStatus nsb_update_density_grid(NsbContext* c, const NsbGridUpdate*
 		a.rng_state = u->rng_state; a.rng_inc = u->rng_inc;
 		for (int k = 0; k < 3; ++k) { a.amin[k] = u->train_aabb_min[k]; a.amax[k] = u->train_aabb_max[k]; }
 		a.density_activation = u->density_activation; a.apply_ops = u->apply_operators ? 1 : 0;
-		uint32_t grid = (n_total + 127u) / 128u;
-		uint32_t cap = (uint32_t)(c->sm_count * c->grid_update_ctas_per_sm);
-		if (grid > cap) grid = cap;
-		(c->acc16 ? k_density_grid_update<true> : k_density_grid_update<false>)<<<grid, 128, sizeof(tc::TileSmem), st>>>(c->model, c->d_ops.get(), c->n_ops, a, c->d_density_grid.get(), c->d_density_tmp.get());
+		(c->acc16 ? k_density_grid_update<true> : k_density_grid_update<false>)<<<tile_ctas(c, n_total, c->grid_update_ctas_per_sm), 128, sizeof(tc::TileSmem), st>>>(c->model, c->d_ops.get(), c->n_ops, a, c->d_density_grid.get(), c->d_density_tmp.get());
 	}
 	k_ema_grid<<<(NSB_GRID_CELLS + 255) / 256, 256, 0, st>>>((uint32_t)NSB_GRID_CELLS, u->decay, c->d_density_grid.get(), c->d_density_tmp.get());  // :3634
 	CU(cudaGetLastError());
@@ -1557,9 +1561,7 @@ extern "C" NsbStatus nsb_poisson_boundary(NsbContext* c, const float* points, ui
 	CU(cudaMemcpy(d_coords.get(), coords.data(), (size_t)n * 7 * 4, cudaMemcpyHostToDevice));
 	float aabb[6] = {p->train_aabb_min[0], p->train_aabb_min[1], p->train_aabb_min[2], p->train_aabb_max[0], p->train_aabb_max[1], p->train_aabb_max[2]};
 	CU(cudaMemcpy(d_aabb.get(), aabb, sizeof(aabb), cudaMemcpyHostToDevice));
-	uint32_t grid = n_padded / 128, cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
-	if (grid > cap) grid = cap;
-	(c->acc16 ? k_inference<false, true> : k_inference<false, false>)<<<grid, 128, sizeof(tc::TileSmem)>>>(c->model, d_coords.get(), n, d_net.get(), n_padded);  // inference_mixed_precision (:2286)
+	(c->acc16 ? k_inference<false, true> : k_inference<false, false>)<<<tile_ctas(c, n_padded, c->inference_ctas_per_sm), 128, sizeof(tc::TileSmem)>>>(c->model, d_coords.get(), n, d_net.get(), n_padded);  // inference_mixed_precision (:2286)
 	const float scale = (float)(4 * M_PI / (double)n_sh);                                                // :2341
 	nsb::rebuild::k_boundary_fit<<<n_points, 32>>>(d_net.get(), n_padded, d_coords.get(), n_sh, p->rgb_activation, p->density_activation,
 	                                               p->is_inside ? c->d_bitfield.get() : nullptr, d_aabb.get(), scale, d_dens.get(), d_shs.get());
@@ -1970,10 +1972,7 @@ static NsbStatus inference_impl(NsbContext* c, const float* coords, uint32_t n, 
 	if (n_padded == 0) return NSB_OK;  // empty batch
 	if (!coords || !out) return fail(NSB_ERR_INVALID, "null argument");
 	CU(cudaSetDevice(c->device));
-	uint32_t grid = n_padded / 128;
-	uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
-	if (grid > cap) grid = cap;
-	(c->acc16 ? k_inference<DENSITY_ONLY, true> : k_inference<DENSITY_ONLY, false>)<<<grid, 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(c->model, coords, n, reinterpret_cast<__half*>(out), n_padded);
+	(c->acc16 ? k_inference<DENSITY_ONLY, true> : k_inference<DENSITY_ONLY, false>)<<<tile_ctas(c, n_padded, c->inference_ctas_per_sm), 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(c->model, coords, n, reinterpret_cast<__half*>(out), n_padded);
 	CU(cudaGetLastError());
 	return NSB_OK;
 }
@@ -2093,12 +2092,6 @@ static mesh::GridQuery grid_query(const NsbGridQuery* q) {
 	}
 	return g;
 }
-// one 128-point tile per CTA, at most the resident CTAs of the operator-level kernels
-static uint32_t grid_ctas(const NsbContext* c, const mesh::GridQuery& g) {
-	const uint32_t grid = next_multiple_u32(g.res[0] * g.res[1] * g.res[2], 128u) / 128;
-	const uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
-	return grid > cap ? cap : grid;
-}
 
 extern "C" NsbStatus nsb_density_on_grid(NsbContext* c, const NsbGridQuery* q, float* density_dev, void* stream) {
 	if (!c || !q || !density_dev) return fail(NSB_ERR_INVALID, "null argument");
@@ -2107,7 +2100,8 @@ extern "C" NsbStatus nsb_density_on_grid(NsbContext* c, const NsbGridQuery* q, f
 	if (!grid_res_ok(q->res)) return fail(NSB_ERR_INVALID, "nsb_density_on_grid: res must be positive multiples of 16 with a 32-bit point count");
 	CU(cudaSetDevice(c->device));
 	const mesh::GridQuery g = grid_query(q);
-	(c->acc16 ? mesh::k_density_on_grid<true> : mesh::k_density_on_grid<false>)<<<grid_ctas(c, g), 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(
+	const uint64_t n = (uint64_t)g.res[0] * g.res[1] * g.res[2];
+	(c->acc16 ? mesh::k_density_on_grid<true> : mesh::k_density_on_grid<false>)<<<tile_ctas(c, n, c->inference_ctas_per_sm), 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(
 		c->model, g, c->d_density_grid.get(), density_dev);
 	CU(cudaGetLastError());
 	return NSB_OK;
@@ -2198,10 +2192,7 @@ extern "C" NsbStatus nsb_mesh_shade(NsbContext* c, const float* train_aabb_min, 
 	                                                        c->mesh_normals.get());
 	mesh::Aabb train;
 	for (int a = 0; a < 3; ++a) { train.mn[a] = train_aabb_min[a]; train.mx[a] = train_aabb_max[a]; }
-	uint32_t grid = rows / 128;
-	const uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
-	if (grid > cap) grid = cap;
-	(c->acc16 ? mesh::k_mesh_colors<true> : mesh::k_mesh_colors<false>)<<<grid, 128, sizeof(tc::TileSmem), st>>>(
+	(c->acc16 ? mesh::k_mesh_colors<true> : mesh::k_mesh_colors<false>)<<<tile_ctas(c, rows, c->inference_ctas_per_sm), 128, sizeof(tc::TileSmem), st>>>(
 		c->model, rows, c->mesh_verts.get(), train, rgb_activation, linear_colors ? 1 : 0, c->mesh_colors.get());
 	CU(cudaGetLastError());
 	c->mesh_shaded = c->mesh_normals_ok = true;
@@ -2245,10 +2236,7 @@ extern "C" NsbStatus nsb_density_gradient(NsbContext* c, const float* coords, ui
 	io.in = coords; io.n = n; io.n_padded = n_padded;
 	io.grad = grad; io.grad_stride = grad_stride_floats;
 	io.dens = reinterpret_cast<__half*>(density_fp16); io.dfeat = reinterpret_cast<__half*>(dfeat_fp16);
-	uint32_t grid = (n_padded + 127) / 128;
-	const uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
-	if (grid > cap) grid = cap;
-	(c->acc16 ? meshopt::k_density_gradient<true, false> : meshopt::k_density_gradient<false, false>)<<<grid, 128, sizeof(meshopt::GradSmem), (cudaStream_t)stream>>>(
+	(c->acc16 ? meshopt::k_density_gradient<true, false> : meshopt::k_density_gradient<false, false>)<<<tile_ctas(c, n_padded, c->inference_ctas_per_sm), 128, sizeof(meshopt::GradSmem), (cudaStream_t)stream>>>(
 		c->model, io);
 	CU(cudaGetLastError());
 	return NSB_OK;
@@ -2285,9 +2273,7 @@ extern "C" NsbStatus nsb_mesh_optimise(NsbContext* c, const NsbMeshOptimise* p, 
 	io.dfeat = nullptr;
 	for (int a = 0; a < 3; ++a) { io.train.mn[a] = p->train_aabb_min[a]; io.train.mx[a] = p->train_aabb_max[a]; }
 	const meshopt::OptParams op{p->thresh, p->smooth_amount, p->density_amount, p->inflate_amount};
-	uint32_t grid = rows / 128;
-	const uint32_t cap = (uint32_t)(c->sm_count * c->inference_ctas_per_sm);
-	if (grid > cap) grid = cap;
+	const uint32_t grid = tile_ctas(c, rows, c->inference_ctas_per_sm);
 	auto grad_kernel = c->acc16 ? meshopt::k_density_gradient<true, true> : meshopt::k_density_gradient<false, true>;
 	for (uint32_t s = 0; s < n_steps; ++s) {
 		io.in = c->mesh_verts.get();
@@ -2315,7 +2301,8 @@ extern "C" NsbStatus nsb_rgba_on_grid(NsbContext* c, const NsbGridQuery* q, cons
 	if ((uintptr_t)rgba_dev & 15u) return fail(NSB_ERR_INVALID, "nsb_rgba_on_grid: rgba_dev must be 16-byte aligned");
 	CU(cudaSetDevice(c->device));
 	const mesh::GridQuery g = grid_query(q);
-	(c->acc16 ? slices::k_rgba_on_grid<true> : slices::k_rgba_on_grid<false>)<<<grid_ctas(c, g), 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(
+	const uint64_t n = (uint64_t)g.res[0] * g.res[1] * g.res[2];
+	(c->acc16 ? slices::k_rgba_on_grid<true> : slices::k_rgba_on_grid<false>)<<<tile_ctas(c, n, c->inference_ctas_per_sm), 128, sizeof(tc::TileSmem), (cudaStream_t)stream>>>(
 		c->model, g, ray_dir[0], ray_dir[1], ray_dir[2], rgb_activation, density_activation, reinterpret_cast<float4*>(rgba_dev));
 	CU(cudaGetLastError());
 	return NSB_OK;

@@ -1,5 +1,5 @@
 // Mesh extraction on the device: the kernels behind nsb_density_on_grid, nsb_marching_cubes and nsb_mesh_shade.
-// Included by nsb_kernels.cu after the network kernels (encode_to_a32, tc::run_network, linear_to_srgb).
+// Included by nsb_kernels.cu after the network kernels (network_tiles, linear_to_srgb).
 //
 //   k_density_on_grid      Testbed::get_density_on_grid (testbed_nerf.cu:4538-4586): generate_grid_samples_nerf_uniform (:402-413)
 //                          + NerfNetwork::density + grid_samples_half_to_float (:465-481) in one pass, no position buffer
@@ -33,40 +33,32 @@ struct GridQuery {
 };
 
 // ---- density on a grid ---------------------------------------------------------------------------------------------
-// x fastest. pos = x * (1/res) * (max - min) + min, with the product and sum contracted into one FMA as nvcc compiles the
-// reference's Eigen expression; the network reads the warped position; the filter looks the running density grid up at the
-// unwarped one (grid_samples_half_to_float with m_aabb).
+// Grid point i of the query, x fastest: pos = x * (1/res) * (max - min) + min, with the product and sum contracted into one FMA as
+// nvcc compiles the reference's Eigen expression.
+__device__ __forceinline__ V3 grid_point(const GridQuery& q, uint32_t i) {
+	const uint32_t rxy = q.res[0] * q.res[1];
+	const uint32_t z = i / rxy, r = i - z * rxy, y = r / q.res[0], x = r - y * q.res[0];
+	return v3(fma_(mul((float)x, q.inv_res[0]), q.rext[0], q.rmin[0]), fma_(mul((float)y, q.inv_res[1]), q.rext[1], q.rmin[1]),
+	          fma_(mul((float)z, q.inv_res[2]), q.rext[2], q.rmin[2]));
+}
+
+// The network reads the warped grid point; the filter looks the running density grid up at the unwarped one (grid_samples_half_to_float
+// with m_aabb).
 template <bool ACC16>
 __global__ void __launch_bounds__(128) k_density_on_grid(const DevModel m, const GridQuery q, const float* __restrict__ density_grid, float* __restrict__ out) {
-	extern __shared__ __align__(128) uint8_t smem_raw[];
-	tc::TileSmem& S = *reinterpret_cast<tc::TileSmem*>(smem_raw);
-	const uint32_t tid = threadIdx.x;
-	tc::tile_setup(S, m.w_image);
-	const uint32_t rxy = q.res[0] * q.res[1];
-	const uint32_t n = rxy * q.res[2];
+	const uint32_t n = q.res[0] * q.res[1] * q.res[2];
 	const uint32_t n_padded = ((n + 127u) / 128u) * 128u;  // the host checks that this fits 32 bits
-	for (uint32_t base = blockIdx.x * 128u; base < n_padded; base += gridDim.x * 128u) {
-		const uint32_t i = base + tid;
-		const bool valid = i < n;
-		V3 pw = v3(0, 0, 0);
-		const V3 dw = v3(0.5f, 0.5f, 0.5f);  // the density MLP does not read the direction
-		if (valid) {
-			const uint32_t z = i / rxy, r = i - z * rxy, y = r / q.res[0], x = r - y * q.res[0];
-			const V3 p = v3(fma_(mul((float)x, q.inv_res[0]), q.rext[0], q.rmin[0]), fma_(mul((float)y, q.inv_res[1]), q.rext[1], q.rmin[1]),
-			                fma_(mul((float)z, q.inv_res[2]), q.rext[2], q.rmin[2]));
-			pw = warp_position(p, q.tmin, q.tmax);
-		}
-		uint32_t dens[8], rgbo[8];
-		encode_to_a32(S.a32, m, valid, pw, tid);
-		tc::run_network<ACC16>(tc::single_tile_ctx(S), dw, true, dens, rgbo);
-		if (valid) {
-			float v = __half2float(__ushort_as_half((unsigned short)(dens[0] & 0xffffu)));  // the raw output, not the activated density
-			const V3 p = unwarp_position(pw, q.tmin, q.tmax);
-			const uint32_t mip = (uint32_t)mip_from_pos(p);
-			if (__ldg(density_grid + cascaded_grid_idx_at(p, mip) + mip * GRIDVOL) < 0.01f) v = -10000.0f;  // NERF_MIN_OPTICAL_THICKNESS
-			out[i] = v;
-		}
-	}
+	// the density MLP does not read the direction
+	network_tiles<ACC16>(m, n, n_padded, true, v3(0.5f, 0.5f, 0.5f), [&](uint32_t i, V3& pw, V3&) {
+		pw = warp_position(grid_point(q, i), q.tmin, q.tmax);
+	}, [&](uint32_t i, bool valid, V3 pw, const uint32_t* dens, const uint32_t*) {
+		if (!valid) return;
+		float v = __half2float(__ushort_as_half((unsigned short)(dens[0] & 0xffffu)));  // the raw output, not the activated density
+		const V3 p = unwarp_position(pw, q.tmin, q.tmax);
+		const uint32_t mip = (uint32_t)mip_from_pos(p);
+		if (__ldg(density_grid + cascaded_grid_idx_at(p, mip) + mip * GRIDVOL) < 0.01f) v = -10000.0f;  // NERF_MIN_OPTICAL_THICKNESS
+		out[i] = v;
+	});
 }
 
 // ---- marching cubes ------------------------------------------------------------------------------------------------
@@ -286,23 +278,19 @@ struct Aabb { float mn[3], mx[3]; };
 
 // ---- vertex colours ------------------------------------------------------------------------------------------------
 // dir = normalize(pos - 0.5) (Eigen normalized(): unchanged when the norm is 0), the network at {warp(pos), warp(dir)}, then
-// network_to_rgb and, for linear colours, linear_to_srgb; every row including the padding (whose position is the origin)
+// network_to_rgb and, for linear colours, linear_to_srgb; every row including the padding (whose position is the origin), so n_rows
+// (a multiple of 128) rows are all valid
 template <bool ACC16>
 __global__ void __launch_bounds__(128) k_mesh_colors(const DevModel m, uint32_t n_rows, const float* __restrict__ verts, const Aabb train,
                                                      int rgb_activation, int linear_colors, float* __restrict__ colors) {
-	extern __shared__ __align__(128) uint8_t smem_raw[];
-	tc::TileSmem& S = *reinterpret_cast<tc::TileSmem*>(smem_raw);
-	const uint32_t tid = threadIdx.x;
-	tc::tile_setup(S, m.w_image);
-	for (uint32_t base = blockIdx.x * 128u; base < n_rows; base += gridDim.x * 128u) {  // n_rows is a multiple of 128
-		const uint32_t i = base + tid;
+	network_tiles<ACC16>(m, n_rows, n_rows, false, v3(0.5f, 0.5f, 0.5f), [&](uint32_t i, V3& pw, V3& dw) {
 		const V3 p = ldv(verts, i);
 		V3 d = vsub(p, v3(0.5f, 0.5f, 0.5f));
 		const float n2 = dot3(d, d);
 		if (n2 > 0.0f) { const float nn = __fsqrt_rn(n2); d = v3(div_(d.x, nn), div_(d.y, nn), div_(d.z, nn)); }
-		uint32_t dens[8], rgbo[8];
-		encode_to_a32(S.a32, m, true, warp_position(p, train.mn, train.mx), tid);
-		tc::run_network<ACC16>(tc::single_tile_ctx(S), warp_direction(d), false, dens, rgbo);
+		pw = warp_position(p, train.mn, train.mx);
+		dw = warp_direction(d);
+	}, [&](uint32_t i, bool, V3, const uint32_t*, const uint32_t* rgbo) {
 		const unsigned short h[3] = {(unsigned short)(rgbo[0] & 0xffffu), (unsigned short)(rgbo[0] >> 16), (unsigned short)(rgbo[1] & 0xffffu)};
 #pragma unroll
 		for (int k = 0; k < 3; ++k) {
@@ -310,7 +298,7 @@ __global__ void __launch_bounds__(128) k_mesh_colors(const DevModel m, uint32_t 
 			if (linear_colors) c = linear_to_srgb(c);
 			colors[3 * (size_t)i + k] = c;
 		}
-	}
+	});
 }
 
 }  // namespace mesh

@@ -1,5 +1,5 @@
 // Density and RGBA slices on the device: the kernels behind nsb_rgba_on_grid, nsb_density_png and nsb_rgba_png.
-// Included by nsb_kernels.cu after nsb_mesh.cuh (mesh::GridQuery, encode_to_a32, tc::run_network).
+// Included by nsb_kernels.cu after nsb_mesh.cuh (mesh::GridQuery, mesh::grid_point, network_tiles).
 //
 //   k_rgba_on_grid   Testbed::get_rgba_on_grid (testbed_nerf.cu:4588-4612): generate_grid_samples_nerf_uniform_dir (:416-427)
 //                    + NerfNetwork::inference + compute_nerf_density (:624-635) in one pass, no position buffer, no 1M batches
@@ -8,44 +8,27 @@
 namespace slices {
 
 // ---- RGBA on a grid ------------------------------------------------------------------------------------------------
-// x fastest over the query's box. The position is the one k_density_on_grid computes: the PTX of the reference's
-// generate_grid_samples_nerf_uniform_dir contracts x * (1/res) * (max - min) + min into mul + fma like its uniform variant.
+// The positions are mesh::grid_point's: the PTX of the reference's generate_grid_samples_nerf_uniform_dir contracts
+// x * (1/res) * (max - min) + min into mul + fma like its uniform variant. One direction for the whole launch.
 // The network output rows 0-3 (rgb, then the density via extract_density) become float as tcnn's float inference output does;
 // then compute_nerf_density: a = clamp(1 - __expf(-network_to_density(d) / 100), 0, 1) with div.rn, rgb = network_to_rgb(c) * a.
 template <bool ACC16>
 __global__ void __launch_bounds__(128) k_rgba_on_grid(const DevModel m, const mesh::GridQuery q, float dx, float dy, float dz, int rgb_act, int density_act,
                                                       float4* __restrict__ out) {
-	extern __shared__ __align__(128) uint8_t smem_raw[];
-	tc::TileSmem& S = *reinterpret_cast<tc::TileSmem*>(smem_raw);
-	const uint32_t tid = threadIdx.x;
-	tc::tile_setup(S, m.w_image);
-	const V3 dw = warp_direction(v3(dx, dy, dz));
-	const uint32_t rxy = q.res[0] * q.res[1];
-	const uint32_t n = rxy * q.res[2];
+	const uint32_t n = q.res[0] * q.res[1] * q.res[2];
 	const uint32_t n_padded = ((n + 127u) / 128u) * 128u;  // the host checks that this fits 32 bits
-	for (uint32_t base = blockIdx.x * 128u; base < n_padded; base += gridDim.x * 128u) {
-		const uint32_t i = base + tid;
-		const bool valid = i < n;
-		V3 pw = v3(0, 0, 0);
-		if (valid) {
-			const uint32_t z = i / rxy, r = i - z * rxy, y = r / q.res[0], x = r - y * q.res[0];
-			const V3 p = v3(fma_(mul((float)x, q.inv_res[0]), q.rext[0], q.rmin[0]), fma_(mul((float)y, q.inv_res[1]), q.rext[1], q.rmin[1]),
-			                fma_(mul((float)z, q.inv_res[2]), q.rext[2], q.rmin[2]));
-			pw = warp_position(p, q.tmin, q.tmax);
-		}
-		uint32_t dens[8], rgbo[8];
-		encode_to_a32(S.a32, m, valid, pw, tid);
-		tc::run_network<ACC16>(tc::single_tile_ctx(S), dw, false, dens, rgbo);
-		if (valid) {
-			const float d = __half2float(__ushort_as_half((unsigned short)(dens[0] & 0xffffu)));
-			const float a = clampf(sub(1.0f, __expf(div_(-network_to_density(d, density_act), 100.0f))), 0.0f, 1.0f);
-			const unsigned short h[3] = {(unsigned short)(rgbo[0] & 0xffffu), (unsigned short)(rgbo[0] >> 16), (unsigned short)(rgbo[1] & 0xffffu)};
-			float c[3];
+	network_tiles<ACC16>(m, n, n_padded, false, warp_direction(v3(dx, dy, dz)), [&](uint32_t i, V3& pw, V3&) {
+		pw = warp_position(mesh::grid_point(q, i), q.tmin, q.tmax);
+	}, [&](uint32_t i, bool valid, V3, const uint32_t* dens, const uint32_t* rgbo) {
+		if (!valid) return;
+		const float d = __half2float(__ushort_as_half((unsigned short)(dens[0] & 0xffffu)));
+		const float a = clampf(sub(1.0f, __expf(div_(-network_to_density(d, density_act), 100.0f))), 0.0f, 1.0f);
+		const unsigned short h[3] = {(unsigned short)(rgbo[0] & 0xffffu), (unsigned short)(rgbo[0] >> 16), (unsigned short)(rgbo[1] & 0xffffu)};
+		float c[3];
 #pragma unroll
-			for (int k = 0; k < 3; ++k) c[k] = mul(network_to_rgb(__half2float(__ushort_as_half(h[k])), rgb_act), a);
-			out[i] = make_float4(c[0], c[1], c[2], a);
-		}
-	}
+		for (int k = 0; k < 3; ++k) c[k] = mul(network_to_rgb(__half2float(__ushort_as_half(h[k])), rgb_act), a);
+		out[i] = make_float4(c[0], c[1], c[2], a);
+	});
 }
 
 // ---- slice images --------------------------------------------------------------------------------------------------

@@ -27,6 +27,15 @@ def _torch():
     return torch
 
 
+def _grid_query(res3d, aabb, train_aabb) -> abi.NsbGridQuery:
+    """The NsbGridQuery of density_on_grid and rgba_on_grid: res3d points over aabb, warped with train_aabb."""
+    q = abi.NsbGridQuery()
+    q.res[:] = [int(v) for v in res3d]
+    q.aabb_min[:], q.aabb_max[:] = [float(v) for v in aabb[0]], [float(v) for v in aabb[1]]
+    q.train_aabb_min[:], q.train_aabb_max[:] = [float(v) for v in train_aabb[0]], [float(v) for v in train_aabb[1]]
+    return q
+
+
 class NerfRenderer:
     def __init__(self, device: int | None = None):
         torch = _torch()
@@ -321,10 +330,7 @@ class NerfRenderer:
         """Testbed::get_density_on_grid: float32 CUDA tensor [res_z, res_y, res_x] (x fastest) of raw densities, -10000 where the running
         density grid is empty. res3d: positive multiples of 16."""
         torch = _torch()
-        q = abi.NsbGridQuery()
-        q.res[:] = [int(v) for v in res3d]
-        q.aabb_min[:], q.aabb_max[:] = [float(v) for v in aabb[0]], [float(v) for v in aabb[1]]
-        q.train_aabb_min[:], q.train_aabb_max[:] = [float(v) for v in train_aabb[0]], [float(v) for v in train_aabb[1]]
+        q = _grid_query(res3d, aabb, train_aabb)
         if out is None:
             out = torch.empty((max(q.res[2], 0), max(q.res[1], 0), max(q.res[0], 0)), dtype=torch.float32, device=torch.device("cuda", self.device))
         s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
@@ -394,10 +400,7 @@ class NerfRenderer:
         """Testbed::get_rgba_on_grid: float32 CUDA tensor [res_z, res_y, res_x, 4] (x fastest) of compute_nerf_density's premultiplied
         rgb and alpha, the network seen from ray_dir at the grid positions of density_on_grid over aabb. res3d: positive multiples of 16."""
         torch = _torch()
-        q = abi.NsbGridQuery()
-        q.res[:] = [int(v) for v in res3d]
-        q.aabb_min[:], q.aabb_max[:] = [float(v) for v in aabb[0]], [float(v) for v in aabb[1]]
-        q.train_aabb_min[:], q.train_aabb_max[:] = [float(v) for v in train_aabb[0]], [float(v) for v in train_aabb[1]]
+        q = _grid_query(res3d, aabb, train_aabb)
         d = (C.c_float * 3)(*[float(v) for v in ray_dir])
         if out is None:
             out = torch.empty((max(q.res[2], 0), max(q.res[1], 0), max(q.res[0], 0), 4), dtype=torch.float32, device=torch.device("cuda", self.device))
