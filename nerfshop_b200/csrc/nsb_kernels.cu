@@ -157,14 +157,17 @@ __device__ __forceinline__ void encode_to_a32(uint8_t* a32, const DevModel& m, b
 // direction; the other rows keep the origin and dw_default. emit(i, valid, pw, dens, rgbo) runs for every row i < n_padded, the
 // padding included, with the network's outputs (density_only: the density MLP alone). n_padded must be a multiple of 128: emit is
 // called for every row of every tile, so a partial last tile would reach past n_padded.
+// The loop walks tile indices, not row bases: a row base stepped by gridDim.x * 128 wraps past 2^32 when n_padded is within one stride
+// of it, and the CTA would start over. A tile index stays below 2^25 and its step below 2^16, so it cannot wrap.
 template <bool ACC16, typename Sample, typename Emit>
 __device__ __forceinline__ void network_tiles(const DevModel& m, uint32_t n, uint32_t n_padded, bool density_only, V3 dw_default, Sample sample, Emit emit) {
 	extern __shared__ __align__(128) uint8_t smem_raw[];
 	tc::TileSmem& S = *reinterpret_cast<tc::TileSmem*>(smem_raw);
 	const uint32_t tid = threadIdx.x;
 	tc::tile_setup(S, m.w_image);
-	for (uint32_t base = blockIdx.x * 128u; base < n_padded; base += gridDim.x * 128u) {
-		const uint32_t i = base + tid;
+	const uint32_t n_tiles = n_padded / 128u;
+	for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+		const uint32_t i = t * 128u + tid;
 		const bool valid = i < n;
 		V3 pw = v3(0, 0, 0), dw = dw_default;
 		if (valid) sample(i, pw, dw);

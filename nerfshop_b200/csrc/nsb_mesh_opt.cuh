@@ -70,8 +70,10 @@ __global__ void __launch_bounds__(128) k_density_gradient(const DevModel m, cons
 	__syncthreads();
 	const uint32_t a32 = tc::smem_u32(S.t.a32), w = tc::smem_u32(S.t.w), wt = tc::smem_u32(S.wt);
 	const __half2 g_scale = __floats2half2_rn(128.0f, 128.0f), zero = __floats2half2_rn(0.0f, 0.0f);
-	for (uint32_t base = blockIdx.x * 128u; base < io.n_padded; base += gridDim.x * 128u) {
-		const uint32_t i = base + tid;
+	// tile indices, as network_tiles walks them (a row base would wrap past 2^32 for n_padded near it)
+	const uint32_t n_tiles = (uint32_t)(((uint64_t)io.n_padded + 127u) / 128u);
+	for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+		const uint32_t i = t * 128u + tid;
 		const bool valid = i < io.n;
 		V3 pw = v3(0, 0, 0);
 		if (valid) pw = VERTS ? warp_position(ldv(io.in, i), io.train.mn, io.train.mx) : v3(io.in[7 * (size_t)i], io.in[7 * (size_t)i + 1], io.in[7 * (size_t)i + 2]);
