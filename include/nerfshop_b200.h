@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define NSB_ABI_VERSION 6
+#define NSB_ABI_VERSION 7
 
 /* reference: common_nerf.h:16-39 */
 #define NSB_NERF_GRIDSIZE 128u
@@ -378,6 +378,21 @@ NsbStatus nsb_cage_deform(NsbContext* ctx, int32_t op_index, const float* cage_v
  * lut_offsets [NSB_GRID_CELLS+1], lut_idx [idx_capacity >= *n_idx], boxes [12] = bbox min,max, warped bbox min,max. */
 NsbStatus nsb_cage_download(NsbContext* ctx, int32_t op_index, float* vertices, float* rotations, uint32_t* lut_offsets, uint32_t* lut_idx,
                             uint64_t idx_capacity, uint64_t* n_idx, float* boxes);
+/* replaces TetMesh::vanish (tet_mesh.cu:251-363, clear_grid :239-248), the cage tool's "Vanish!" button (growing_selection.cu:184-194), for the
+ * cage operator op_index of the uploaded list: every cell, at each of the 5 cascades, that one of the operator's CURRENT tets touches
+ * (its vertices as nsb_set_edit_ops uploaded them or the last nsb_cage_deform rebuilt them; the cell test of build_tet_grid: a cell corner
+ * inside the tet or a tet face hitting the cell box) gets density 0.0f in the context's running density grid and its bit cleared in the
+ * context's occupancy bitfield, at its own cascade. The grid mean, the max-pooled coarser cascades, the EMA step and the rng are left as
+ * they are, as vanish leaves them. The next nsb_render sees the result.
+ * Differences from the reference: a context with a bitfield (nsb_upload_occupancy) but no running density grid has its bitfield
+ * cleared only (the reference always has a grid).
+ * A later nsb_update_density_grid refills vanished cells from the network: the reference's GUI turns auto-clean off after vanishing
+ * for that reason; this library has no auto-clean, so the caller decides when to update. The host's copy of the grid (the reference's
+ * m_nerf.density_grid) is stale until nsb_download_density_grid.
+ * n_cells_cleared (may be NULL): if given, receives the number of cells whose density or bit changed, and the call synchronises
+ * the stream; otherwise it is stream-ordered and does not synchronise. Allocates nothing.
+ * Errors: NSB_ERR_INVALID for an index out of range or an operator that is not a cage with tets, NSB_ERR_STATE without occupancy. */
+NsbStatus nsb_cage_vanish(NsbContext* ctx, int32_t op_index, uint64_t* n_cells_cleared, void* stream);
 
 /* ---- membrane (Poisson) boundary values (SURVEY.md §8f-4) ------------------------------------------------------------ */
 /* The members GrowingSelection::compute_poisson_boundary reads (growing_selection.cu:2220-2348). */

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libnerfshop_b200.so")
 
-NSB_ABI_VERSION = 6
+NSB_ABI_VERSION = 7
 NSB_MLP_ACC_F32, NSB_MLP_ACC_F16 = 0, 1
 NSB_NERF_GRIDSIZE = 128
 NSB_NERF_CASCADES = 5
@@ -141,7 +141,7 @@ class NsbMeshOptimise(C.Structure):
 EXPORTED_SYMBOLS = [
     "nsb_abi_version", "nsb_last_error", "nsb_create", "nsb_destroy",
     "nsb_model_n_params", "nsb_set_mlp_accumulator", "nsb_upload_model", "nsb_upload_model_dev", "nsb_upload_occupancy_dev", "nsb_upload_occupancy", "nsb_upload_density_grid", "nsb_set_edit_ops",
-    "nsb_update_density_grid", "nsb_download_density_grid", "nsb_cage_attach_mvc", "nsb_cage_deform", "nsb_cage_download",
+    "nsb_update_density_grid", "nsb_download_density_grid", "nsb_cage_attach_mvc", "nsb_cage_deform", "nsb_cage_download", "nsb_cage_vanish",
     "nsb_poisson_boundary", "nsb_cage_set_membrane",
     "nsb_render", "nsb_render_host", "nsb_render_host_async", "nsb_host_frame_wait", "nsb_get_stats", "nsb_debug_counters",
     "nsb_tiles_for_rank", "nsb_pack_tiles", "nsb_unpack_tiles", "nsb_unpack_gathered", "nsb_accumulate", "nsb_tonemap",
@@ -195,6 +195,7 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.nsb_cage_attach_mvc.argtypes = [vp, i32, vp, u32]
     lib.nsb_cage_deform.argtypes = [vp, i32, vp, u32, vp]
     lib.nsb_cage_download.argtypes = [vp, i32, vp, vp, vp, vp, u64, C.POINTER(u64), vp]
+    lib.nsb_cage_vanish.argtypes = [vp, i32, C.POINTER(u64), vp]
     lib.nsb_poisson_boundary.argtypes = [vp, vp, u32, C.POINTER(NsbBoundarySampling), vp, vp]
     lib.nsb_cage_set_membrane.argtypes = [vp, i32, vp, u32, vp, vp, vp, vp, f32, i32, vp, vp, vp]
     lib.nsb_set_edit_ops.argtypes = [vp, C.POINTER(NsbEditOp), i32]

@@ -136,6 +136,50 @@ __global__ void k_local_rotations(const float* __restrict__ verts, const float* 
 	tet_rotation(verts, orig, tets + 4 * (size_t)t, rots + 9 * (size_t)t);
 }
 
+// ---- the cell box of one (tet, cascade) and the cell test of build_tet_grid and vanish (tet_mesh.cu:278-330, :407-460) -------------
+// Loads tet t's vertices into v and returns the number of cells of its box at `level`: first cell lo, extents (.., ny, nz), half cell
+// size h. (v stays a separate array: the face loop indexes it dynamically, so it lives in local memory, and nothing else should.)
+__device__ __forceinline__ uint32_t tet_cell_box(const float* __restrict__ verts, const uint32_t* __restrict__ tets, uint32_t t, uint32_t level, P3* v, int* lo,
+                                                 uint32_t& ny, uint32_t& nz, float& h) {
+	for (int j = 0; j < 4; ++j) v[j] = pld(verts, tets[4 * t + j]);
+	P3 mn = v[0], mx = v[0];
+	for (int j = 1; j < 4; ++j) {
+		mn = p3(fminf(mn.x, v[j].x), fminf(mn.y, v[j].y), fminf(mn.z, v[j].z));
+		mx = p3(fmaxf(mx.x, v[j].x), fmaxf(mx.y, v[j].y), fmaxf(mx.z, v[j].z));
+	}
+	int hi[3];
+	get_cell_at_pos(mn, level, lo);
+	get_cell_at_pos(mx, level, hi);
+	const uint32_t nx = (uint32_t)(hi[0] - lo[0] + 1);
+	ny = (uint32_t)(hi[1] - lo[1] + 1);
+	nz = (uint32_t)(hi[2] - lo[2] + 1);
+	const uint32_t n_cells = nx * ny * nz;
+	const float scale = pow2f((int)level);
+	h = div_(mul(0.5f, scale), 128.0f);
+	return n_cells;
+}
+// Cell c of the box: its coordinates, and whether the tet touches it (a cell corner inside the tet, or a tet face hitting the cell box).
+__device__ __forceinline__ bool tet_touches_cell(const P3* v, const int* lo, uint32_t ny, uint32_t nz, float h, uint32_t c, uint32_t level, uint32_t& x,
+                                                 uint32_t& y, uint32_t& z) {
+	x = (uint32_t)lo[0] + c / (ny * nz); y = (uint32_t)lo[1] + (c / nz) % ny; z = (uint32_t)lo[2] + c % nz;
+	const P3 ctr = get_cell_pos(x, y, z, level);
+	bool inside = false;
+#pragma unroll 1
+	for (int k = 0; k < 8 && !inside; ++k) {
+		// corner order of the host code; +-0.5 * scale / 128 is exact
+		const float sx = (k == 3 || k == 4 || k == 6 || k == 7) ? h : -h;
+		const float sy = (k == 2 || k == 4 || k == 5 || k == 7) ? h : -h;
+		const float sz = (k == 1 || k == 5 || k == 6 || k == 7) ? h : -h;
+		inside = point_in_tet(v, p3(add(ctr.x, sx), add(ctr.y, sy), add(ctr.z, sz)));
+	}
+	if (!inside) {
+		const P3 bmin = p3(sub(ctr.x, h), sub(ctr.y, h), sub(ctr.z, h)), bmax = p3(add(ctr.x, h), add(ctr.y, h), add(ctr.z, h));
+#pragma unroll 1
+		for (int j = 0; j < 4 && !inside; ++j) inside = box_intersects_triangle(bmin, bmax, v[j], v[(j + 1) & 3], v[(j + 2) & 3]);
+	}
+	return inside;
+}
+
 // ---- TetMesh::build_tet_grid, pass 1: one CTA per (tet, cascade); its threads stride over the cells of the tet's box -----------
 struct Mark { uint32_t cell, tet; };
 __global__ void __launch_bounds__(128) k_tet_mark(const float* __restrict__ verts, const uint32_t* __restrict__ tets, uint32_t n_tets, uint32_t* __restrict__ counts,
@@ -143,43 +187,50 @@ __global__ void __launch_bounds__(128) k_tet_mark(const float* __restrict__ vert
 	const uint32_t t = blockIdx.x / CASCADES, level = blockIdx.x % CASCADES;
 	if (t >= n_tets) return;
 	P3 v[4];
-	for (int j = 0; j < 4; ++j) v[j] = pld(verts, tets[4 * t + j]);
-	P3 mn = v[0], mx = v[0];
-	for (int j = 1; j < 4; ++j) {
-		mn = p3(fminf(mn.x, v[j].x), fminf(mn.y, v[j].y), fminf(mn.z, v[j].z));
-		mx = p3(fmaxf(mx.x, v[j].x), fmaxf(mx.y, v[j].y), fmaxf(mx.z, v[j].z));
-	}
-	int lo[3], hi[3];
-	get_cell_at_pos(mn, level, lo);
-	get_cell_at_pos(mx, level, hi);
-	const uint32_t nx = (uint32_t)(hi[0] - lo[0] + 1), ny = (uint32_t)(hi[1] - lo[1] + 1), nz = (uint32_t)(hi[2] - lo[2] + 1);
-	const uint32_t n_cells = nx * ny * nz;
-	const float scale = pow2f((int)level);
-	const float h = div_(mul(0.5f, scale), 128.0f);
+	int lo[3];
+	uint32_t ny, nz;
+	float h;
+	const uint32_t n_cells = tet_cell_box(verts, tets, t, level, v, lo, ny, nz, h);
 	for (uint32_t c = threadIdx.x; c < n_cells; c += blockDim.x) {
-		const uint32_t x = (uint32_t)lo[0] + c / (ny * nz), y = (uint32_t)lo[1] + (c / nz) % ny, z = (uint32_t)lo[2] + c % nz;
-		const P3 ctr = get_cell_pos(x, y, z, level);
-		bool inside = false;
-#pragma unroll 1
-		for (int k = 0; k < 8 && !inside; ++k) {
-			// corner order of the host code; +-0.5 * scale / 128 is exact
-			const float sx = (k == 3 || k == 4 || k == 6 || k == 7) ? h : -h;
-			const float sy = (k == 2 || k == 4 || k == 5 || k == 7) ? h : -h;
-			const float sz = (k == 1 || k == 5 || k == 6 || k == 7) ? h : -h;
-			inside = point_in_tet(v, p3(add(ctr.x, sx), add(ctr.y, sy), add(ctr.z, sz)));
-		}
-		if (!inside) {
-			const P3 bmin = p3(sub(ctr.x, h), sub(ctr.y, h), sub(ctr.z, h)), bmax = p3(add(ctr.x, h), add(ctr.y, h), add(ctr.z, h));
-#pragma unroll 1
-			for (int j = 0; j < 4 && !inside; ++j) inside = box_intersects_triangle(bmin, bmax, v[j], v[(j + 1) & 3], v[(j + 2) & 3]);
-		}
-		if (inside) {
+		uint32_t x, y, z;
+		if (tet_touches_cell(v, lo, ny, nz, h, c, level, x, y, z)) {
 			const uint32_t cell = level * GRIDVOL + morton3D(x, y, z);
 			atomicAdd(counts + cell, 1u);
 			const unsigned int pos = atomicAdd(n_marks, 1u);
 			if (pos < marks_cap) { marks[pos].cell = cell; marks[pos].tet = t; }
 		}
 	}
+}
+
+// ---- TetMesh::vanish (tet_mesh.cu:251-363) and clear_grid (:239-248): k_tet_mark's launch shape and cell test ------------------
+// Every touched cell's density becomes 0 (grid may be null) and its occupancy bit is cleared with an atomicAnd on the 32-bit word that
+// holds it: many CTAs clear bits of one word, where the reference clears from one thread. Clearing is idempotent, so a cell touched by
+// several tets needs no dedup. A counted call (n_cleared != null) with a grid takes two launches so that each changed cell counts once:
+// the first (mark_nonzero) zeroes the densities and SETS the bit of every cell whose density was not 0, the second (grid == null) clears
+// the bits and counts those it found set.
+__global__ void __launch_bounds__(128) k_tet_vanish(const float* __restrict__ verts, const uint32_t* __restrict__ tets, uint32_t n_tets, float* __restrict__ grid,
+                                                    uint32_t* __restrict__ bits, int mark_nonzero, unsigned long long* __restrict__ n_cleared) {
+	const uint32_t t = blockIdx.x / CASCADES, level = blockIdx.x % CASCADES;
+	if (t >= n_tets) return;
+	P3 v[4];
+	int lo[3];
+	uint32_t ny, nz;
+	float h;
+	const uint32_t n_cells = tet_cell_box(verts, tets, t, level, v, lo, ny, nz, h);
+	uint32_t n = 0;
+	for (uint32_t c = threadIdx.x; c < n_cells; c += blockDim.x) {
+		uint32_t x, y, z;
+		if (!tet_touches_cell(v, lo, ny, nz, h, c, level, x, y, z)) continue;
+		const uint32_t cell = level * GRIDVOL + morton3D(x, y, z), mask = 1u << (cell & 31u);  // byte cell/8, bit cell%8 = word cell/32, bit cell%32
+		if (mark_nonzero) {
+			if (__float_as_uint(atomicExch(grid + cell, 0.0f)) != 0u) atomicOr(bits + (cell >> 5), mask);
+			continue;
+		}
+		if (grid) grid[cell] = 0.0f;
+		if (n_cleared) n += (atomicAnd(bits + (cell >> 5), ~mask) & mask) != 0u;
+		else atomicAnd(bits + (cell >> 5), ~mask);
+	}
+	if (n) atomicAdd(n_cleared, (unsigned long long)n);
 }
 
 // ---- exclusive scan of the per-cell counts (3 launches: block sums, scan of block sums, block scans + offset) -------------------

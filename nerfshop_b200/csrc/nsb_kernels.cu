@@ -1016,6 +1016,7 @@ struct NsbContext {
 	};
 	std::vector<CageArrays> rb;
 	DevBuf<uint32_t> d_counters;       // [0] rays queued by k_prepare_rays, [1] fetch cursor of k_render_fused
+	DevBuf<unsigned long long> d_n_cleared;  // cells a counted nsb_cage_vanish changed
 	DevBuf<unsigned long long> d_stats;
 	DevBuf<RayRec> d_list;
 	DevBuf<float> d_ray_od;            // origin + direction per queue slot, general-camera frames only (allocated on the first such frame)
@@ -1092,6 +1093,7 @@ extern "C" NsbStatus nsb_create(int device, NsbContext** out) {
 	c->device = device;
 	c->sm_count = prop.multiProcessorCount;
 	CU(c->d_counters.reserve(2));
+	CU(c->d_n_cleared.reserve(1));
 	CU(c->d_stats.reserve(ST_N));
 	CU(cudaMemset(c->d_stats.get(), 0, ST_N * sizeof(unsigned long long)));
 	CU(cudaEventCreate(&c->ev0));
@@ -1516,6 +1518,34 @@ extern "C" NsbStatus nsb_cage_deform(NsbContext* c, int32_t op_index, const floa
 	cp3(d.bmin, boxes); cp3(d.bmax, boxes + 3); cp3(d.wbmin, boxes + 6); cp3(d.wbmax, boxes + 9);
 	CU(cudaMemcpyAsync(c->d_ops.get() + op_index, &d, sizeof(DevOp), cudaMemcpyHostToDevice, s));
 	CU(cudaGetLastError());
+	return NSB_OK;
+}
+// TetMesh::vanish (tet_mesh.cu:251-363): the cells the operator's current (deformed) tets touch leave the context's running density grid and
+// occupancy bitfield, on the stream, with nothing allocated and nothing synchronised unless the count is asked for
+extern "C" NsbStatus nsb_cage_vanish(NsbContext* c, int32_t op_index, uint64_t* n_cells_cleared, void* stream_) {
+	using namespace nsb::rebuild;
+	NsbStatus st = cage_slot(c, op_index, "nsb_cage_vanish");
+	if (st != NSB_OK) return st;
+	if (!c->has_occ || !c->d_bitfield.get()) return fail(NSB_ERR_STATE, "nsb_cage_vanish: no occupancy (nsb_upload_occupancy, nsb_upload_density_grid or nsb_update_density_grid)");
+	CU(cudaSetDevice(c->device));
+	cudaStream_t s = (cudaStream_t)stream_;
+	const DevOp& d = c->h_ops[op_index];
+	float* grid = c->d_density_grid.get();
+	uint32_t* bits = reinterpret_cast<uint32_t*>(c->d_bitfield.get());
+	const uint32_t n_ctas = d.n_tets * CASCADES;
+	if (!n_cells_cleared) {
+		k_tet_vanish<<<n_ctas, 128, 0, s>>>(d.verts, d.tets, d.n_tets, grid, bits, 0, nullptr);
+		CU(cudaGetLastError());
+		return NSB_OK;
+	}
+	unsigned long long* d_n = c->d_n_cleared.get();
+	CU(cudaMemsetAsync(d_n, 0, sizeof(*d_n), s));
+	if (grid) k_tet_vanish<<<n_ctas, 128, 0, s>>>(d.verts, d.tets, d.n_tets, grid, bits, 1, nullptr);
+	k_tet_vanish<<<n_ctas, 128, 0, s>>>(d.verts, d.tets, d.n_tets, nullptr, bits, 0, d_n);
+	unsigned long long n = 0;
+	CU(cudaMemcpyAsync(&n, d_n, sizeof(n), cudaMemcpyDeviceToHost, s));
+	CU(cudaStreamSynchronize(s));
+	*n_cells_cleared = n;
 	return NSB_OK;
 }
 // ---- membrane boundary values (SURVEY.md §8f-4) ---------------------------------------------------------------------

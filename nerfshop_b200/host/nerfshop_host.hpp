@@ -142,6 +142,9 @@ public:
 	// GrowingSelection::update_tet_mesh for operator i after a gizmo drag (growing_selection.cu:1615): no re-upload.
 	void attach_mvc(size_t i, const float* mvc_weights, uint32_t n_cage_vertices) { check(nsb_cage_attach_mvc(m_ctx->get(), (int32_t)i, mvc_weights, n_cage_vertices), "nsb_cage_attach_mvc"); }
 	void deform_cage(size_t i, const float* cage_vertices, uint32_t n_cage_vertices, void* stream) { check(nsb_cage_deform(m_ctx->get(), (int32_t)i, cage_vertices, n_cage_vertices, stream), "nsb_cage_deform"); }
+	// TetMesh::vanish (tet_mesh.cu:251-363), the cage tool's "Vanish!" button: clears the cells operator i's tets cover in the context's
+	// density grid and occupancy, stream-ordered. A later update_density_grid refills them from the network.
+	void vanish_cage(size_t i, void* stream) { check(nsb_cage_vanish(m_ctx->get(), (int32_t)i, nullptr, stream), "nsb_cage_vanish"); }
 	// GrowingSelection::interpolate_poisson_boundary (growing_selection.cu:2350-2398)
 	void set_membrane(size_t i, const float* gamma, uint32_t n_cage_vertices, const float* d_in, const float* d_out, const float* shs_in, const float* shs_out, float amplitude, bool apply) {
 		check(nsb_cage_set_membrane(m_ctx->get(), (int32_t)i, gamma, n_cage_vertices, d_in, d_out, shs_in, shs_out, amplitude, apply ? 1 : 0, nullptr, nullptr, nullptr), "nsb_cage_set_membrane");

@@ -121,6 +121,14 @@ class NerfRenderer:
         cv = np.ascontiguousarray(cage_vertices, np.float32).reshape(-1, 3)
         abi.check(self.lib, self.lib.nsb_cage_deform(self.ctx, op_index, cv.ctypes.data, cv.shape[0], stream), "nsb_cage_deform")
 
+    def cage_vanish(self, op_index: int, count: bool = False, stream: int = 0):
+        """TetMesh::vanish (tet_mesh.cu:251-363): zero the density and clear the occupancy bit of every cell, at every cascade, that the
+        cage operator's current tets touch. Stream-ordered; with count=True it synchronises and returns the number of cells whose density or
+        bit changed. A later update_density_grid refills the cells from the network."""
+        n = C.c_uint64()
+        abi.check(self.lib, self.lib.nsb_cage_vanish(self.ctx, op_index, C.byref(n) if count else None, stream), "nsb_cage_vanish")
+        return int(n.value) if count else None
+
     def cage_download(self, op_index: int, n_vertices: int, n_tets: int, rotations: bool = True) -> dict:
         n = C.c_uint64()
         abi.check(self.lib, self.lib.nsb_cage_download(self.ctx, op_index, None, None, None, None, 0, C.byref(n), None), "nsb_cage_download")
