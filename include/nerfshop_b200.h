@@ -178,6 +178,8 @@ typedef struct {
 	const float*    boundary_shs;              /* [27*n_vertices] SH9RGB column-major (9 x 3), or NULL */
 	const float*    boundary_outside_density;  /* [n_vertices] or NULL */
 	const float*    boundary_residual_density; /* [n_vertices] or NULL */
+	/* The render's membrane residuals use an operator only when all three boundary arrays are given; the density-grid residual
+	 * (nsb_poisson_residual_density, the occupancy update) needs only boundary_residual_density. */
 
 	/* ---- affine ---- */
 	NsbAffineBox selection_box;    /* m_warped_selection_box */

@@ -647,11 +647,11 @@ __global__ void k_map_positions(const DevOp* __restrict__ ops, int n_ops, float*
 }
 
 // The loop of compute_poisson_residual_density_kernel (cage_deformation.cu:341-383): h += (half) interpolated residual density, for the
-// first tet that contains the (warped) position pw, of each operator in reverse order
+// first tet that contains the (warped) position pw, of each operator in reverse order. Only the residual density array is required (:647-672).
 __device__ __forceinline__ void add_residual_density(const DevOp* __restrict__ ops, int n_ops, V3 pw, __half& h) {
 	for (int o = n_ops - 1; o >= 0; --o) {
 		const DevOp& op = ops[o];
-		if (op.type != 0 || !op.apply_poisson || !op.has_poisson_data || op.n_tets == 0) continue;
+		if (op.type != 0 || !op.apply_poisson || !op.rd || op.n_tets == 0) continue;
 		V3 p = unwarp_position(pw, op.amin, op.amax);
 		if (!box_contains(op.bmin, op.bmax, p)) continue;
 		float b[4];
@@ -1382,12 +1382,12 @@ extern "C" NsbStatus nsb_set_edit_ops(NsbContext* c, const NsbEditOp* ops, int32
 				if ((st = dev_copy(r.orig_verts, s.original_vertices, (size_t)3 * s.n_vertices, &d.orig_verts)) != NSB_OK) return st;
 				if ((st = dev_copy(r.rots, s.local_rotations, (size_t)9 * s.n_tets, &d.rots)) != NSB_OK) return st;
 				if ((st = dev_copy(r.obits, s.original_bitfield, (size_t)NSB_BITFIELD_BYTES, &d.obits)) != NSB_OK) return st;
-				if (s.boundary_shs && s.boundary_outside_density && s.boundary_residual_density) {
-					if ((st = dev_copy(r.shs, s.boundary_shs, (size_t)27 * s.n_vertices, &d.shs)) != NSB_OK) return st;
-					if ((st = dev_copy(r.od, s.boundary_outside_density, (size_t)s.n_vertices, &d.od)) != NSB_OK) return st;
-					if ((st = dev_copy(r.rd, s.boundary_residual_density, (size_t)s.n_vertices, &d.rd)) != NSB_OK) return st;
-					d.has_poisson_data = 1;
-				}
+				// each membrane array may come alone: the density-grid residual needs only boundary_residual_density (cage_deformation.cu:647-672),
+				// the render's full residuals need all three (:675-716)
+				if ((st = dev_copy(r.shs, s.boundary_shs, (size_t)27 * s.n_vertices, &d.shs)) != NSB_OK) return st;
+				if ((st = dev_copy(r.od, s.boundary_outside_density, (size_t)s.n_vertices, &d.od)) != NSB_OK) return st;
+				if ((st = dev_copy(r.rd, s.boundary_residual_density, (size_t)s.n_vertices, &d.rd)) != NSB_OK) return st;
+				d.has_poisson_data = d.shs && d.od && d.rd;
 				if (d.apply_poisson && d.has_poisson_data) any_poisson = 1;
 			}
 		} else if (s.type == NSB_OP_AFFINE) {

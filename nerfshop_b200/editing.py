@@ -181,13 +181,12 @@ class CageDeformation:
         if self.use_local_rotations:
             op.local_rotations = _fptr(keep["rot"])
         op.original_bitfield = keep["bits"].ctypes.data_as(C.POINTER(C.c_uint8))
-        if self.boundary_shs is not None:
-            keep["shs"] = np.ascontiguousarray(self.boundary_shs.reshape(-1))
-            keep["od"] = self.boundary_outside_density
-            keep["rd"] = self.boundary_residual_density
-            op.boundary_shs = _fptr(keep["shs"])
-            op.boundary_outside_density = _fptr(keep["od"])
-            op.boundary_residual_density = _fptr(keep["rd"])
+        # each membrane array may be absent on its own (NULL)
+        for name, field, arr in (("shs", "boundary_shs", self.boundary_shs), ("od", "boundary_outside_density", self.boundary_outside_density),
+                                 ("rd", "boundary_residual_density", self.boundary_residual_density)):
+            if arr is not None:
+                keep[name] = np.ascontiguousarray(arr, np.float32).reshape(-1)
+                setattr(op, field, _fptr(keep[name]))
         return op, keep
 
 

@@ -610,11 +610,60 @@ void map_one(const NsbEditOp* ops, int n_ops, V3& pos_w, V3& dir_w, bool& empty)
 		else affine_map(ops[i], pos_w, dir_w, empty);
 	}
 }
+// EditOperator::map_positions for one position, operators in reverse list order (testbed_nerf.cu:3595-3598): interpolate_tet_pos
+// (cage_deformation.cu:136-192: no direction, and the vacated-region mask does not look at `copy`) and translate_in_box_pos
+// (affine_duplication.cu:69-90: no direction)
+void map_position_one(const NsbEditOp* ops, int n_ops, V3& pos_w, bool& empty) {
+	for (int i = n_ops - 1; i >= 0; --i) {
+		const NsbEditOp& op = ops[i];
+		V3 d = v3(0.5f, 0.5f, 0.5f);
+		if (op.type == NSB_OP_CAGE) {
+			NsbEditOp pos_only = op;
+			pos_only.copy = 0;
+			pos_only.local_rotations = nullptr;
+			cage_map(pos_only, pos_w, d, empty);
+		} else {
+			NsbEditOp pos_only = op;
+			pos_only.correct_dir = 0;
+			affine_map(pos_only, pos_w, d, empty);
+		}
+	}
+}
+// EditOperator::compute_poisson_residual_density for one position, operators in reverse list order (testbed_nerf.cu:3612-3620): the loop of
+// compute_poisson_residual_density_kernel (cage_deformation.cu:341-383), h += (half) interpolated residual density, for the first tet of each
+// operator that contains the (mapped, warped) position. Gated like CageDeformation::compute_poisson_residual_density (:647-672): only the
+// residual density array has to be present. Returns how many operators added a residual; *last is the last one added.
+int add_residual_density_one(const NsbEditOp* ops, int n_ops, V3 pos_w, uint16_t& h, uint16_t* last) {
+	int n = 0;
+	for (int k = n_ops - 1; k >= 0; --k) {
+		const NsbEditOp& op = ops[k];
+		if (op.type != NSB_OP_CAGE || !op.apply_poisson || op.n_tets == 0 || !op.boundary_residual_density) continue;
+		Box saabb = mkbox(op.scene_aabb_min, op.scene_aabb_max);
+		Box bbox = mkbox(op.bbox_min, op.bbox_max);
+		V3 q = unwarp_position(pos_w, saabb);
+		if (!box_contains(bbox, q)) continue;
+		float b[4];
+		int t = find_tet(op, q, b);
+		if (t < 0) continue;
+		const uint32_t* tv = op.tets + 4 * (size_t)t;
+		float res = fmaf(b[3], op.boundary_residual_density[tv[3]], fmaf(b[2], op.boundary_residual_density[tv[2]],
+		            fmaf(b[0], op.boundary_residual_density[tv[0]], b[1] * op.boundary_residual_density[tv[1]])));
+		uint16_t r = f2h(res);
+		if (last) *last = r;
+		++n;
+		h = hadd(h, r);                                                                              // half += half (:379)
+	}
+	return n;
+}
+// CageDeformation::compute_poisson_full_residuals gates on all three membrane arrays (cage_deformation.cu:675-716)
+inline bool has_full_membrane(const NsbEditOp& op) {
+	return op.type == NSB_OP_CAGE && op.apply_poisson && op.n_tets != 0 && op.boundary_shs && op.boundary_outside_density && op.boundary_residual_density;
+}
 // compute_residual_poisson_kernel (cage_deformation.cu:431-541) for one sample; outputs pre-zeroed by the caller.
 void poisson_one(const NsbEditOp* ops, int n_ops, V3 pos_w, float* sh27, float* out_density, float* residual_density) {
 	for (int i = n_ops - 1; i >= 0; --i) { // testbed_nerf.cu:2868
 		const NsbEditOp& op = ops[i];
-		if (op.type != NSB_OP_CAGE || !op.apply_poisson || op.n_tets == 0 || !op.boundary_shs) continue; // :686
+		if (!has_full_membrane(op)) continue;
 		Box aabb = mkbox(op.scene_aabb_min, op.scene_aabb_max);
 		Box bbox = mkbox(op.bbox_min, op.bbox_max);
 		V3 p = unwarp_position(pos_w, aabb);
@@ -1008,6 +1057,31 @@ int orc_poisson_residuals(const OrcScene* s, const float* coords, uint32_t n, fl
 	}
 	return 0;
 }
+// EditOperator::map_positions over all operators: positions (warped) are `stride` floats apart, mapped in place; the mask (optional) is only
+// ever set, like nsb_map_positions for one operator.
+int orc_map_positions(const OrcScene* s, float* positions, uint32_t stride, uint8_t* empty_mask, uint32_t n) {
+	if (stride < 3) return 1;
+#pragma omp parallel for schedule(static)
+	for (int64_t i = 0; i < (int64_t)n; ++i) {
+		float* q = positions + (size_t)i * stride;
+		V3 p = v3(q[0], q[1], q[2]);
+		bool empty = false;
+		map_position_one(s->ops, s->n_ops, p, empty);
+		q[0] = p.x; q[1] = p.y; q[2] = p.z;
+		if (empty && empty_mask) empty_mask[i] = 1;
+	}
+	return 0;
+}
+// EditOperator::compute_poisson_residual_density over all operators: density_fp16[i] += each operator's residual density at position i
+int orc_poisson_residual_density(const OrcScene* s, const float* positions, uint32_t stride, uint16_t* density_fp16, uint32_t n) {
+	if (stride < 3) return 1;
+#pragma omp parallel for schedule(static)
+	for (int64_t i = 0; i < (int64_t)n; ++i) {
+		const float* q = positions + (size_t)i * stride;
+		add_residual_density_one(s->ops, s->n_ops, v3(q[0], q[1], q[2]), density_fp16[i], nullptr);
+	}
+	return 0;
+}
 
 // Occupancy march without termination. rec: n_pixels*max_samples*5 floats (t, dt, x, y, z);
 // idx: n_pixels*max_samples*2 (mip, cell); count: total occupied samples on the ray.
@@ -1055,7 +1129,7 @@ int orc_render(const OrcScene* s, const NsbFrame* f, float* fb, float* depth, Or
 	const Box train = mkbox(f->train_aabb_min, f->train_aabb_max);
 	const bool ops_on = f->apply_operators && s->n_ops > 0;
 	bool any_poisson = false;
-	if (ops_on) for (int i = 0; i < s->n_ops; ++i) any_poisson |= (s->ops[i].type == NSB_OP_CAGE && s->ops[i].apply_poisson && s->ops[i].boundary_shs);
+	if (ops_on) for (int i = 0; i < s->n_ops; ++i) any_poisson |= has_full_membrane(s->ops[i]);
 	uint64_t n_alive = 0, n_hit = 0, n_samples = 0, n_old = 0;
 	const V3 cam_fwd = v3(f->camera1[6], f->camera1[7], f->camera1[8]);
 	const V3 cam_org = v3(f->camera1[9], f->camera1[10], f->camera1[11]);
@@ -1356,33 +1430,14 @@ int orc_update_density_grid(const OrcScene* s, const NsbGridUpdate* u, float* gr
 		V3 pw = warp_position(p, aabb);
 		if (u->apply_operators && s->n_ops > 0) {                                               // map_positions, reverse order (:3593-3599)
 			bool empty = false;
-			V3 d = v3(0.5f, 0.5f, 0.5f);
-			map_one(s->ops, s->n_ops, pw, d, empty);
+			map_position_one(s->ops, s->n_ops, pw, empty);
 		}
 		uint16_t o[16], d16[16];
 		network_forward(m, pw, v3(0.5f, 0.5f, 0.5f), o, d16, true);                             // NerfNetwork::density (:3601-3603)
 		uint16_t h = f2h(network_to_density(h2f(d16[0]), u->density_activation));               // activate_network_density (:3522-3531)
 		uint16_t residual = 0;
 		int n_residuals = 0;
-		if (u->apply_operators) {
-			for (int k = s->n_ops - 1; k >= 0; --k) {                                           // compute_poisson_residual_density (:3612-3620)
-				const NsbEditOp& op = s->ops[k];
-				if (op.type != NSB_OP_CAGE || !op.apply_poisson || op.n_tets == 0 || !op.boundary_residual_density) continue;
-				Box saabb = mkbox(op.scene_aabb_min, op.scene_aabb_max);
-				Box bbox = mkbox(op.bbox_min, op.bbox_max);
-				V3 q = unwarp_position(pw, saabb);                                              // the MAPPED position (cage_deformation.cu:358-359)
-				if (!box_contains(bbox, q)) continue;
-				float b[4];
-				int t = find_tet(op, q, b);
-				if (t < 0) continue;
-				const uint32_t* tv = op.tets + 4 * (size_t)t;
-				float res = fmaf(b[3], op.boundary_residual_density[tv[3]], fmaf(b[2], op.boundary_residual_density[tv[2]],
-				            fmaf(b[0], op.boundary_residual_density[tv[0]], b[1] * op.boundary_residual_density[tv[1]])));
-				residual = f2h(res);
-				++n_residuals;
-				h = hadd(h, residual);                                                          // half += half (:379)
-			}
-		}
+		if (u->apply_operators) n_residuals = add_residual_density_one(s->ops, s->n_ops, pw, h, &residual);  // at the MAPPED position (:3612-3620)
 		const float ot = h2f(h) * MIN_STEP();                                                   // splat_..._already_activated (:447-463)
 		uint32_t ob;
 		memcpy(&ob, &ot, 4);

@@ -67,6 +67,8 @@ def lib() -> C.CDLL:
         l.orc_inference.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_uint32, C.c_void_p, C.c_int]
         l.orc_map_rays.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_void_p, C.c_uint32]
         l.orc_poisson_residuals.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
+        l.orc_map_positions.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+        l.orc_poisson_residual_density.argtypes = [C.POINTER(OrcScene), C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
         l.orc_march_trace.argtypes = [C.POINTER(OrcScene), C.POINTER(abi.NsbFrame), C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
         l.orc_render.argtypes = [C.POINTER(OrcScene), C.POINTER(abi.NsbFrame), C.c_void_p, C.c_void_p, C.POINTER(OrcStats), C.c_void_p]
         l.orc_set_threads.argtypes = [C.c_int]
@@ -147,6 +149,21 @@ class Oracle:
         rd = np.zeros(n, np.float32)
         assert self.lib.orc_poisson_residuals(C.byref(self.scene), _ptr(c), n, _ptr(sh), _ptr(od), _ptr(rd)) == 0
         return sh, od, rd
+
+    def map_positions(self, positions: np.ndarray, mask: np.ndarray | None = None):
+        """EditOperator::map_positions over all operators. positions: float32 [n, stride >= 3], warped position in the first 3 columns
+        (mapped in place on a copy). mask: uint8 [n] that the operators may only set, or None. Returns (positions, mask)."""
+        p = np.ascontiguousarray(positions, np.float32).copy()
+        m = None if mask is None else np.ascontiguousarray(mask, np.uint8).copy()
+        assert self.lib.orc_map_positions(C.byref(self.scene), _ptr(p), p.shape[1], None if m is None else _ptr(m), p.shape[0]) == 0
+        return p, m
+
+    def poisson_residual_density(self, positions: np.ndarray, density_fp16: np.ndarray) -> np.ndarray:
+        """EditOperator::compute_poisson_residual_density over all operators: density_fp16 (uint16 bits [n]) plus the residuals at positions [n, stride]."""
+        p = np.ascontiguousarray(positions, np.float32)
+        h = np.ascontiguousarray(density_fp16).view(np.uint16).copy()
+        assert self.lib.orc_poisson_residual_density(C.byref(self.scene), _ptr(p), p.shape[1], _ptr(h), p.shape[0]) == 0
+        return h
 
     def march_trace(self, frame: abi.NsbFrame, pixels: np.ndarray, max_samples: int):
         pixels = np.ascontiguousarray(pixels, np.uint32)

@@ -54,6 +54,16 @@ def lib() -> C.CDLL:
     return _lib
 
 
+# entry points added to ref_driver.cpp after libraries that may still be in use were built: where the reference's sources are absent, a
+# prebuilt library is used as it is and may lack them
+_LATER = {"map_positions": "ref_map_positions", "poisson_residual_density": "ref_poisson_residual_density"}
+
+
+def serves(name: str) -> bool:
+    """The loaded library has the entry point behind this module's function `name`."""
+    return name not in _LATER or hasattr(lib(), _LATER[name])
+
+
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
 
@@ -315,6 +325,28 @@ def poisson_residuals(ops, coords):
     arr, n_ops = _ops_array(ops)
     assert lib().ref_poisson_residuals(arr, n_ops, _p(c), n, _p(sh), _p(od), _p(rd)) == 0
     return sh, od, rd
+
+
+def map_positions(ops, positions, mask):
+    """EditOperator::map_positions of every operator, reverse list order. positions [n, stride] (warped position first), mask uint8 [n]."""
+    p = f32(positions).copy()
+    m = np.ascontiguousarray(mask, np.uint8).copy()
+    arr, n_ops = _ops_array(ops)
+    l = lib()
+    l.ref_map_positions.argtypes = [C.POINTER(abi.NsbEditOp), C.c_int, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+    assert l.ref_map_positions(arr, n_ops, _p(p), p.shape[1], _p(m), p.shape[0]) == 0
+    return p, m
+
+
+def poisson_residual_density(ops, positions, density_fp16):
+    """EditOperator::compute_poisson_residual_density of every operator, reverse list order: density_fp16 (uint16 bits) plus the residuals."""
+    p = f32(positions).copy()
+    h = np.ascontiguousarray(density_fp16).view(np.uint16).copy()
+    arr, n_ops = _ops_array(ops)
+    l = lib()
+    l.ref_poisson_residual_density.argtypes = [C.POINTER(abi.NsbEditOp), C.c_int, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+    assert l.ref_poisson_residual_density(arr, n_ops, _p(p), p.shape[1], _p(h), p.shape[0]) == 0
+    return h
 
 
 def compute_mvc(cage_vertices, cage_tris, points, gamma=1.0, original=True):

@@ -346,6 +346,23 @@ int ref_poisson_residuals(const NsbEditOp* ops, int n_ops, const float* coords, 
 	for (uint32_t i = 0; i < n; ++i) memcpy(sh + 27 * (size_t)i, shs[i].data(), 27 * sizeof(float));
 	return 0;
 }
+// ---- EditOperator::map_positions / compute_poisson_residual_density on a flat batch (reverse list order, testbed_nerf.cu:3595-3598, 3612-3620) ----
+// positions: warped, `stride` floats apart; empty_mask: in/out (only ever set). density: fp16 bits, in/out.
+int ref_map_positions(const NsbEditOp* ops, int n_ops, float* positions, uint32_t stride, uint8_t* empty_mask, uint32_t n) {
+	static_assert(sizeof(NerfPosition) == 3 * sizeof(float), "NerfPosition layout");
+	GPUMatrix<bool> mask(1, n);
+	for (uint32_t i = 0; i < n; ++i) mask.data()[i] = empty_mask[i] != 0;
+	PitchedPtr<NerfPosition> in((NerfPosition*)positions, 0, 0, (size_t)stride * sizeof(float));
+	for (int i = n_ops - 1; i >= 0; --i) make_op(ops[i])->map_positions(nullptr, in, mask, n);
+	for (uint32_t i = 0; i < n; ++i) empty_mask[i] = mask.data()[i] ? 1 : 0;
+	return 0;
+}
+int ref_poisson_residual_density(const NsbEditOp* ops, int n_ops, float* positions, uint32_t stride, uint16_t* density, uint32_t n) {
+	static_assert(sizeof(tcnn::network_precision_t) == sizeof(uint16_t), "fp16 density");
+	PitchedPtr<NerfPosition> in((NerfPosition*)positions, 0, 0, (size_t)stride * sizeof(float));
+	for (int i = n_ops - 1; i >= 0; --i) make_op(ops[i])->compute_poisson_residual_density(nullptr, n, in, (tcnn::network_precision_t*)density);
+	return 0;
+}
 
 // ---- per-edit geometry: MVC (mvc.h:126-188 through Cage::compute_mvc), Kabsch rotations (tet_mesh.cu:38-74 + svd3.h), LUT build ----
 // weights: [n_points x n_cage_vertices] row-major

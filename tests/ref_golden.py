@@ -5,6 +5,8 @@ runs the reference build; with NSB_RECORD_REF_GOLDEN=1 its results are also stor
 tests/golden/ref/<test module>/<test>.npz. Where it does not exist (the reference's sources are not part of this repository),
 the stored results of the same test are replayed, so every comparison still runs against what the reference computed.
 
+A prebuilt library older than one of the entry points (ref.serves) replays that entry point's stored results the same way.
+
 Results too large to store whole keep a fixed, seeded subset of their rows (axis 0: rays, coordinates, grid cells, image rows);
 arrays of one call with the same number of rows keep the same rows. Such a result comes back as a `Sampled` array that knows its
 rows, and `ref.match(ours, theirs)` takes the same rows of this repository's output, so the comparison runs on that sample.
@@ -275,9 +277,9 @@ class _Ref:
 
     def __getattr__(self, name):
         attr = getattr(_ref, name)
-        if not callable(attr) or isinstance(attr, type) or name.startswith("_") or name in ("available", "lib", "cuda_lib", "f32", "u32"):
+        if not callable(attr) or isinstance(attr, type) or name.startswith("_") or name in ("available", "lib", "cuda_lib", "f32", "u32", "serves"):
             return attr
-        return lambda *a, **kw: _call(_HAVE_CPU, attr, *a, **kw)
+        return lambda *a, **kw: _call(_HAVE_CPU and _ref.serves(name), attr, *a, **kw)
 
 
 ref = _Ref()

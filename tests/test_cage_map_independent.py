@@ -1,75 +1,16 @@
 """CPU: an independent numpy restatement of EditOperator::map_rays for a cage (interpolate_tet, cage_deformation.cu:197-269;
 point_in_tet / bary_tet, selection_utils.h:10-47) that does NOT use the lookup table: every tet is tested, the lowest-index containing
-tet wins (= the first entry of the sample's cell list, whose entries are in ascending tet order). Against the oracle's LUT-driven
-map_rays: positions, directions and the empty mask bit for bit. Also pins the LUT's completeness on these samples."""
+tet wins (= the first entry of the sample's cell list, whose entries are in ascending tet order). The rule lives in tests/edit_domain.py
+(map_rays_lut_free). Against the oracle's LUT-driven map_rays: positions, directions and the empty mask bit for bit. Also pins the LUT's
+completeness on these samples."""
 import numpy as np
 
+import edit_domain as ed
 import edit_fixtures as fx
 from conftest import random_coords
 from oracle import oracle as orc
-from test_march_independent import cell_index, mip_from_pos
 
-F32, F64 = np.float32, np.float64
-
-
-def fma(a, b, c):
-    return (np.asarray(a, F64) * np.asarray(b, F64) + np.asarray(c, F64)).astype(F32)
-
-
-def dot3(a, b):   # Eigen's reduction tree x0*y0 + (x1*y1 + x2*y2) as nvcc contracts it: fma(x,x', fma(y,y', z*z'))
-    return fma(a[..., 0], b[..., 0], fma(a[..., 1], b[..., 1], (a[..., 2] * b[..., 2]).astype(F32)))
-
-
-def cross3(a, b):  # fma(a.y, b.z, -(a.z*b.y)), ...
-    return np.stack([fma(a[..., 1], b[..., 2], -(a[..., 2] * b[..., 1]).astype(F32)), fma(a[..., 2], b[..., 0], -(a[..., 0] * b[..., 2]).astype(F32)),
-                     fma(a[..., 0], b[..., 1], -(a[..., 1] * b[..., 0]).astype(F32))], -1)
-
-
-def same_side(v1, v2, v3, v4, p):
-    n = cross3(v2 - v1, v3 - v1)
-    return np.signbit(dot3(n, v4 - v1)) == np.signbit(dot3(n, p - v1))
-
-
-def stp(a, b, c):
-    return dot3(a, cross3(b, c))
-
-
-def map_one(op, pw, dw):
-    """-> (pw', dw', empty)"""
-    mn, mx = op.aabb_min, op.aabb_max
-    diag = mx - mn
-    host, _ = op.to_op()
-    wb = (np.array(host.warped_bbox_min[:], F32), np.array(host.warped_bbox_max[:], F32))
-    ob = (np.array(host.original_warped_bbox_min[:], F32), np.array(host.original_warped_bbox_max[:], F32))
-    in_def = False
-    if (pw >= wb[0]).all() and (pw <= wb[1]).all():
-        p = fma(pw, diag, mn)
-        V = op.vertices[op.tets]                      # [T, 4, 3]
-        a, b, c, d = V[:, 0], V[:, 1], V[:, 2], V[:, 3]
-        inside = same_side(a, b, c, d, p) & same_side(b, c, d, a, p) & same_side(c, d, a, b, p) & same_side(d, a, b, c, p)
-        hit = np.nonzero(inside)[0]
-        if hit.size:
-            t = int(hit[0])
-            a, b, c, d = (V[t, k] for k in range(4))
-            vap, vbp, vab, vac, vad, vbc, vbd = p - a, p - b, b - a, c - a, d - a, c - b, d - b
-            v6 = F32(1.0 / F64(stp(vab, vac, vad)))
-            bary = [stp(vbp, vbd, vbc) * v6, stp(vap, vac, vad) * v6, stp(vap, vad, vab) * v6, stp(vap, vab, vac) * v6]
-            O = op.original_vertices[op.tets[t]]
-            canon = fma(bary[3], O[3], fma(bary[2], O[2], fma(bary[0], O[0], (bary[1] * O[1]).astype(F32))))
-            pw = ((canon - mn) / diag).astype(F32)
-            if op.use_local_rotations:
-                R = op.rotations[t].reshape(3, 3).T   # column-major storage -> R[r][c]
-                ud = fma(dw, F32(2.0), F32(-1.0))
-                rd = np.array([fma(R[r, 0], ud[0], fma(R[r, 1], ud[1], R[r, 2] * ud[2])) for r in range(3)], F32)
-                dw = ((rd + F32(1.0)) * F32(0.5)).astype(F32)
-            in_def = True
-    empty = False
-    if not op.copy and not in_def and (pw >= ob[0]).all() and (pw <= ob[1]).all():
-        p = fma(pw, diag, mn)
-        level = mip_from_pos(p)
-        bitsarr = np.unpackbits(op.original_bitfield, bitorder="little")
-        empty = bool(bitsarr[level * 128 ** 3 + cell_index(p, level)])
-    return pw, dw, empty
+F32 = np.float32
 
 
 def test_numpy_cage_map_equals_the_oracle(scene):
@@ -83,12 +24,8 @@ def test_numpy_cage_map_equals_the_oracle(scene):
     p = centre + (rng.random((n, 3)).astype(F32) * 2 - 1) * half
     c[:, :3] = (p - model.aabb_min) / (model.aabb_max - model.aabb_min)
     ref, mref = o.map_rays(c)
-    moved = masked = 0
-    for i in range(n):
-        pw, dw, empty = map_one(op, c[i, :3].copy(), c[i, 4:].copy())
-        assert np.array_equal(pw.view(np.uint32), ref[i, :3].view(np.uint32)), (i, pw, ref[i, :3])
-        assert np.array_equal(dw.view(np.uint32), ref[i, 4:].view(np.uint32)), (i, dw, ref[i, 4:])
-        assert empty == bool(mref[i])
-        moved += int((pw != c[i, :3]).any())
-        masked += int(empty)
-    assert moved > 100 and masked >= 1
+    got, mgot = ed.map_rays_lut_free([op], c)
+    assert np.array_equal(got.view(np.uint32), ref.view(np.uint32)), np.nonzero((got != ref).any(1))[0][:10]
+    assert np.array_equal(mgot, mref)
+    moved = (got[:, :3] != c[:, :3]).any(1)
+    assert moved.sum() > 100 and mgot.sum() >= 1

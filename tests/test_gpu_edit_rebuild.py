@@ -21,14 +21,15 @@ def _drag(op, pull):
 
 
 def _check_against_host(renderer, op_index, op):
-    got = renderer.cage_download(op_index, op.vertices.shape[0], op.tets.shape[0])
+    got = renderer.cage_download(op_index, op.vertices.shape[0], op.tets.shape[0], rotations=op.use_local_rotations)
     assert np.array_equal(got["vertices"].view(np.uint32), op.vertices.view(np.uint32)), "MVC interpolation must be bit-exact"
     host_op, _ = op.to_op()
     boxes = np.array(list(host_op.bbox_min) + list(host_op.bbox_max) + list(host_op.warped_bbox_min) + list(host_op.warped_bbox_max), np.float32)
     assert np.array_equal(got["boxes"].view(np.uint32), boxes.view(np.uint32))
     assert np.array_equal(got["lut_offsets"], op.lut_offsets), f"{(got['lut_offsets'] != op.lut_offsets).sum()} CSR offsets differ"
     assert np.array_equal(got["lut_idx"], op.lut_idx)
-    assert np.abs(got["rotations"] - op.rotations).max() < 2e-6
+    if op.use_local_rotations:
+        assert np.abs(got["rotations"] - op.rotations).max() < 2e-6
     return got
 
 
