@@ -60,13 +60,14 @@ def get_marching_cubes_res(res_1d: int, aabb) -> np.ndarray:
     return out
 
 
-def grid_positions(res, render_aabb, train_aabb) -> np.ndarray:
-    """generate_grid_samples_nerf_uniform: NerfPosition rows [n, position_floats] (x fastest)."""
+def grid_positions(res, render_aabb, train_aabb, rows=None) -> np.ndarray:
+    """generate_grid_samples_nerf_uniform: NerfPosition rows [n, position_floats] (x fastest); only the given point indices when rows is
+    given (the kernel still runs on the whole grid)."""
     r = np.asarray(res, np.int32)
     out = np.zeros((int(np.prod(r.astype(np.int64))), lib().ref_mesh_position_floats()), np.float32)
     rb, tb = _box(render_aabb), _box(train_aabb)
     _ok(lib().ref_mesh_grid_positions(r.ctypes.data, rb.ctypes.data, tb.ctypes.data, out.ctypes.data), "generate_grid_samples_nerf_uniform")
-    return out
+    return out if rows is None else out[np.asarray(rows, np.int64)]
 
 
 def half_to_float(positions, mlp_u16, train_aabb, density_grid=None) -> np.ndarray:

@@ -32,11 +32,8 @@ def mr(scene, built_lib):
 
 
 def _positions(res):
-    """The grid positions and warped coordinates, exactly: the AABB extent 4 and res are powers of two, so every product is exact."""
-    i = np.arange(res ** 3, dtype=np.int64)
-    xyz = np.stack([i % res, (i // res) % res, i // (res * res)], 1).astype(np.float32)
-    p = xyz * (np.float32(1.0) / np.float32(res)) * np.float32(4.0) + np.float32(-1.5)
-    return p, (p - np.float32(-1.5)) / np.float32(4.0)
+    """The grid positions and warped coordinates of k_density_on_grid (mesh_oracle.grid_positions: fma(x * (1/res), max - min, min))."""
+    return mo.grid_positions((res, res, res), AABB, AABB)
 
 
 def _density(mr, res):
@@ -77,26 +74,16 @@ def test_density_on_grid_equals_nsb_density_with_fp32_accumulators(mr, scene):
 
 def _density_on_grid_equals_nsb_density(mr, scene, policy):
     res = 64
-    p, pw = _positions(res)
+    _, pw = _positions(res)
     coords = np.zeros((pw.shape[0], 7), np.float32)
     coords[:, :3] = pw
     coords[:, 4:] = 0.5
     with _policy(mr, policy):
         got = _density(mr, res)
         raw = mr.density(coords)[0].view(np.float16).astype(np.float32)
-    # cascaded_grid_at(unwarp(warp(p)), density_grid, mip_from_pos) of the occupancy as 0/1: the unwarp is exact here
-    from nerfshop_b200 import synthetic as syn
-
+    # cascaded_grid_at(unwarp(warp(p)), density_grid, mip_from_pos) of the occupancy as 0/1
     model, occ = scene
-    grid = np.unpackbits(occ, bitorder="little")
-    q = p - np.float32(0.5)
-    m = np.abs(q).max(1)
-    mip = np.clip(np.frexp(m)[1] + 1, 0, 4)  # mip_from_pos: frexp exponent + 1
-    mip[m == 0] = 1
-    sc = np.ldexp(np.float32(1.0), 7 - mip).astype(np.float32)
-    c = np.clip(np.floor(q * sc[:, None] + np.float32(64.0)), 0, 127).astype(np.uint32)
-    cell = syn.morton3d(c[:, 0], c[:, 1], c[:, 2]).astype(np.int64) + mip.astype(np.int64) * 128 ** 3
-    empty = grid[cell] == 0
+    empty = mo.filtered(pw, AABB, np.unpackbits(occ, bitorder="little").astype(np.float32))
     assert 0 < empty.sum() < empty.size
     np.testing.assert_array_equal(got[~empty].view(np.uint32), raw[~empty].view(np.uint32))
     assert (got[empty] == -10000.0).all()
@@ -138,27 +125,12 @@ def _normals_and_colours(mr, policy):
         t = _thresh(d0)
         d, m, nv = _mesh(mr, res, t)
     V, N, Cc, F = m["V"], m["N"], m["C"], m["F"].astype(np.int64)
-    # normals: (pb - pa) x (pa - pc) per triangle, summed in triangle order; the device contracts the cross product into FMAs, so
-    # compare in angle
-    pa, pb, pc = V[F[:, 0]].astype(np.float64), V[F[:, 1]].astype(np.float64), V[F[:, 2]].astype(np.float64)
-    tn = np.cross(pb - pa, pa - pc)
-    ref = np.zeros((V.shape[0], 3))
-    for k in range(3):
-        np.add.at(ref, F[:, k], tn)
-    cosang = np.einsum("ij,ij->i", ref[:nv], N[:nv]) / (np.linalg.norm(ref[:nv], axis=1) * np.linalg.norm(N[:nv], axis=1))
-    assert (cosang > 1 - 1e-6).all()
-    # colours: the network at {warp(pos), warp(normalize(pos - 0.5))}; rows where the float64 direction rounds like the device's
-    dd = V.astype(np.float64) - 0.5
-    n = np.sqrt((dd * dd).sum(1))
-    dirs = np.where(n[:, None] > 0, dd / np.where(n > 0, n, 1)[:, None], dd).astype(np.float32)
-    coords = np.zeros((V.shape[0], 7), np.float32)
-    coords[:, :3] = (V - np.float32(-1.5)) / np.float32(4.0)
-    coords[:, 4:] = (dirs + np.float32(1.0)) * np.float32(0.5)
+    # normals: (pb - pa) x (pa - pc) per triangle in its FMA form, summed in ascending triangle order, bit for bit; zero padding rows
+    np.testing.assert_array_equal(mo.bits(N), mo.bits(mo.normals(V, F, nv, V.shape[0])))
+    # colours: the network at {warp(pos), warp(normalize(pos - 0.5))} (mesh_oracle.color_inputs), every row, bit for bit
     with _policy(mr, policy):
-        raw = mr.inference(coords)[:3].view(np.float16).astype(np.float32).T
-    same = (raw == Cc).all(1)
-    assert same.mean() > 0.99  # direction bits may differ in the last place where float64 rounds differently from the FMA form
-    assert np.abs(raw - Cc).max() < 2e-2
+        raw = mr.inference(mo.color_inputs(V, AABB))[:3].view(np.float16).astype(np.float32).T
+    np.testing.assert_array_equal(Cc.view(np.uint32), raw.view(np.uint32))
 
 
 def test_256_mesh_is_edge_manifold_and_reused_context_matches_fresh(mr, scene):
