@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define NSB_ABI_VERSION 7
+#define NSB_ABI_VERSION 8
 
 /* reference: common_nerf.h:16-39 */
 #define NSB_NERF_GRIDSIZE 128u
@@ -519,6 +519,26 @@ NsbStatus nsb_density_png(NsbContext* ctx, const float* density_dev, const int32
  * the reference's file %04d_<w>x<h>.png, each channel (uint8_t)clamp(v * 255, 0, 255); res' and the y flip as nsb_density_png. Needs no
  * model. Stream-ordered. */
 NsbStatus nsb_rgba_png(NsbContext* ctx, const float* rgba_dev, const int32_t res[3], int32_t swap_y_z, uint8_t* pixels_dev, void* stream);
+
+/* ---- whole output frames (ABI 8): Testbed::render_to_cpu (python_api.cu:129-175) and scripts/run.py's --video_camera_path loop ----- */
+/* replaces render_to_cpu's sub-frame loop: for each of the n frames, in order, what Testbed::render_frame (testbed.cu:2632-2765) runs: clear a
+ * frame and depth buffer the context owns (render_buffer.clear_frame), nsb_render into them (the same kernels and instantiation choice), and
+ * nsb_accumulate into accumulate_dev (float4[width*height]) with spp = frames[i].spp_index and tm->color_space (spp 0 clears the buffer first,
+ * so a caller continues a progressive accumulation by starting past 0). Then one nsb_tonemap of accumulate_dev into out_rgba_dev
+ * (float4[width*height]). The result is bit for bit that of the same calls made one by one. All frames have the same size; every frame is
+ * checked as nsb_render checks it (same status codes) and tm as nsb_tonemap does, before anything is enqueued. The two buffers (20 B per
+ * pixel) are allocated on the first call at a size and only grow; nsb_get_stats reports the last sub-frame. Stream-ordered, no host
+ * synchronisation except when one of these buffers, or one of nsb_render's, grows. */
+NsbStatus nsb_render_accumulate(NsbContext* ctx, const NsbFrame* frames, uint32_t n, const NsbTonemap* tm, float* accumulate_dev, float* out_rgba_dev,
+                                void* stream);
+/* replaces scripts/run.py's np.clip(frame * 2**exposure, 0, 1) followed by write_image (scripts/common.py:122-178) for an 8-bit file, on a
+ * DEVICE float4[w*h] frame (16-byte aligned; linear premultiplied RGBA, e.g. nsb_render_accumulate's with output_color_space LINEAR): per
+ * pixel, in float32 with every operation rounded on its own: x = clip(v * 2^exposure, 0, 1) for all four channels; rgb = rgb / a where a != 0,
+ * else 0; rgb = x > 0.0031308 ? 1.055 * x^(1/2.4) - 0.055 : 12.92 * x; byte = (uint8)(clip(x, 0, 1) * 255 + 0.5), NaN giving 0.
+ * out_dev: DEVICE uint8, n_channels = 4: RGBA (4-byte aligned), 3: the same RGB without alpha (what write_image keeps for a JPEG).
+ * powf is CUDA's: a byte may differ from numpy's by one where the float lies within an ulp of a quantisation boundary. Stream-ordered. */
+NsbStatus nsb_frame_to_rgba8(NsbContext* ctx, const float* rgba_dev, int32_t w, int32_t h, float exposure, int32_t n_channels, uint8_t* out_dev,
+                             void* stream);
 
 #ifdef __cplusplus
 }

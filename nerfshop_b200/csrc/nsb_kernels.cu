@@ -932,6 +932,7 @@ __global__ void k_unpack_gathered(const float4* __restrict__ gathered, const flo
 #include "nsb_mesh.cuh"
 #include "nsb_mesh_opt.cuh"
 #include "nsb_slices.cuh"
+#include "nsb_video.cuh"
 
 // =====================================================================================================
 // host side: context, uploads, C ABI
@@ -1025,6 +1026,7 @@ struct NsbContext {
 	bool timed = false;
 	uint32_t launches = 0;
 	DevBuf<float> d_fb, d_depth;       // nsb_render_host
+	DevBuf<float> d_sub_fb, d_sub_depth;  // nsb_render_accumulate: the frame and depth buffers each sub-frame is rendered into
 	cudaStream_t stream = nullptr;
 	// nsb_render_host_async: two framebuffers in flight, the D2H copy of one overlaps the render of the other
 	DevBuf<float> d_fb2[2], d_depth2[2];
@@ -1992,6 +1994,63 @@ extern "C" NsbStatus nsb_tonemap(NsbContext* c, const float* acc, float* out, in
 	CU(cudaSetDevice(c->device));
 	int n = W * H;
 	k_tonemap<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(n, reinterpret_cast<const float4*>(acc), reinterpret_cast<float4*>(out), *p);
+	CU(cudaGetLastError());
+	return NSB_OK;
+}
+
+// ---- whole output frames (ABI 8): Testbed::render_to_cpu's sub-frame loop and run.py's 8-bit conversion ------------------
+// the parameter check nsb_tonemap makes inline (kept there unchanged): the two must stay the same
+static bool tonemap_ok(const NsbTonemap* p) {
+	return p->color_space >= 0 && p->color_space <= 2 && p->output_color_space >= 0 && p->output_color_space <= 1 && p->tonemap_curve >= 0 && p->tonemap_curve <= 3;
+}
+
+extern "C" NsbStatus nsb_render_accumulate(NsbContext* c, const NsbFrame* frames, uint32_t n, const NsbTonemap* tm, float* acc, float* out, void* stream_) {
+	if (!c || !frames || n == 0 || !tm || !acc || !out) return fail(NSB_ERR_INVALID, "null argument or no sub-frames");
+	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_upload_model has not been called");
+	for (uint32_t i = 0; i < n; ++i) {  // every frame as nsb_render checks it, before anything is enqueued
+		DevFrame f;
+		const NsbStatus st = to_dev_frame(&frames[i], &f);
+		if (st != NSB_OK) return fail(st, "nsb_render_accumulate: sub-frame %u: %s", i, g_last_error.c_str());
+		if (frames[i].width != frames[0].width || frames[i].height != frames[0].height)
+			return fail(NSB_ERR_INVALID, "nsb_render_accumulate: sub-frame %u is %dx%d, sub-frame 0 is %dx%d", i, frames[i].width, frames[i].height, frames[0].width, frames[0].height);
+	}
+	if (!tonemap_ok(tm)) return fail(NSB_ERR_INVALID, "bad tonemap parameters");
+	CU(cudaSetDevice(c->device));
+	cudaStream_t stream = (cudaStream_t)stream_;
+	const int W = frames[0].width, H = frames[0].height, np = W * H;
+	const size_t n_px = (size_t)np;
+	if (c->d_sub_fb.capacity() < n_px * 4 || c->d_sub_depth.capacity() < n_px) {  // grows only; the old buffers may still be read on `stream`
+		CU(cudaStreamSynchronize(stream));
+		CU(c->d_sub_fb.reserve(n_px * 4));
+		CU(c->d_sub_depth.reserve(n_px));
+	}
+	float* fb = c->d_sub_fb.get();
+	float* depth = c->d_sub_depth.get();
+	for (uint32_t i = 0; i < n; ++i) {  // render_frame (testbed.cu:2632-2765) per sub-frame: clear_frame, render_nerf, accumulate
+		CU(cudaMemsetAsync(fb, 0, n_px * 16, stream));
+		CU(cudaMemsetAsync(depth, 0, n_px * 4, stream));
+		const NsbStatus st = nsb_render(c, &frames[i], fb, depth, stream);
+		if (st != NSB_OK) return st;
+		const uint32_t spp = frames[i].spp_index;
+		if (spp == 0) CU(cudaMemsetAsync(acc, 0, n_px * 16, stream));  // render_buffer.cu:545-547
+		k_accumulate<<<(np + 255) / 256, 256, 0, stream>>>(np, reinterpret_cast<const float4*>(fb), reinterpret_cast<float4*>(acc), (float)spp, tm->color_space);
+		CU(cudaGetLastError());
+	}
+	k_tonemap<<<(np + 255) / 256, 256, 0, stream>>>(np, reinterpret_cast<const float4*>(acc), reinterpret_cast<float4*>(out), *tm);
+	CU(cudaGetLastError());
+	return NSB_OK;
+}
+
+extern "C" NsbStatus nsb_frame_to_rgba8(NsbContext* c, const float* rgba, int32_t W, int32_t H, float exposure, int32_t n_channels, uint8_t* out, void* stream) {
+	if (!c || !rgba || !out || W <= 0 || H <= 0) return fail(NSB_ERR_INVALID, "bad arguments");
+	if ((uint64_t)W * (uint64_t)H > 0xffffffffull) return fail(NSB_ERR_INVALID, "frame %dx%d has more than 2^32 pixels", W, H);
+	if (n_channels != 3 && n_channels != 4) return fail(NSB_ERR_INVALID, "n_channels must be 3 or 4, not %d", n_channels);
+	if (n_channels == 4 && ((uintptr_t)out & 3u) != 0) return fail(NSB_ERR_INVALID, "a 4-channel output must be 4-byte aligned");
+	if (((uintptr_t)rgba & 15u) != 0) return fail(NSB_ERR_INVALID, "the float4 frame must be 16-byte aligned");
+	CU(cudaSetDevice(c->device));
+	const uint32_t n = (uint32_t)W * (uint32_t)H;
+	const float scale = (float)std::pow(2.0, (double)exposure);  // run.py's 2**exposure: a Python float, rounded to float32 against the float32 frame
+	video::k_rgba8<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(n, reinterpret_cast<const float4*>(rgba), scale, n_channels, out);
 	CU(cudaGetLastError());
 	return NSB_OK;
 }

@@ -10,10 +10,16 @@
 //   ngp_b200::render_nerf(...) <- Testbed::render_nerf      (testbed.h:305, testbed_nerf.cu:3066)
 //   ngp_b200::get_rgba_on_grid, density_png, rgba_png <- Testbed::get_rgba_on_grid and the pixel loops of save_density_grid_to_png /
 //                                                       save_rgba_grid_to_png_sequence (the host keeps its own stbi_write_png)
+//   ngp_b200::CameraKeyframe, CameraPath <- CameraKeyframe / CameraPath (camera_path.h:30-97): keyframe arithmetic and the B-spline path in the
+//                                           reference's float order (no JSON: the host keeps its own load / save)
+//   ngp_b200::render_to_cpu(...)        <- Testbed::render_to_cpu's sub-frame loop (python_api.cu:129-175) and copy back, over
+//                                           nsb_render_accumulate; the caller builds the sub-frames (nerfshop_b200/camera_path.py restates how)
 //
 // Errors become std::runtime_error, as CUDA_CHECK_THROW does in the reference (propagates to main.cu:252).
 #pragma once
 
+#include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <memory>
 #include <stdexcept>
@@ -176,6 +182,95 @@ inline uint32_t render_nerf(NerfTracer& tracer, const NsbFrame& frame, float* fr
 	return tracer.trace(f, frame_buffer_dev, depth_buffer_dev, stream, synchronise);
 }
 
+// CameraKeyframe (camera_path.h:30-62), Eigen-free: R is the quaternion (x, y, z, w). The arithmetic is float, in the order of Eigen's
+// Quaternionf / Vector4f with SSE (a 4-vector's dot product sums (x0 + x2) + (x1 + x3)); compile without FMA contraction to keep it.
+struct CameraKeyframe {
+	float R[4] = {0.f, 0.f, 0.f, 1.f};
+	float T[3] = {0.f, 0.f, 0.f};
+	float slice = 0.f, scale = 1.f, fov = 50.625f, dof = 0.f;
+
+	static float dot4(const float* a, const float* b) { return (a[0] * b[0] + a[2] * b[2]) + (a[1] * b[1] + a[3] * b[3]); }
+	// Quaternionf(R).normalized().toRotationMatrix() and T, as a 3x4 column-major camera (NsbFrame::camera0)
+	void m(float out[12]) const {
+		const float n2 = dot4(R, R);
+		float q[4] = {R[0], R[1], R[2], R[3]};
+		if (n2 > 0.f) for (float& v : q) v = v / std::sqrt(n2);
+		const float x = q[0], y = q[1], z = q[2], w = q[3];
+		const float tx = 2.f * x, ty = 2.f * y, tz = 2.f * z;
+		const float twx = tx * w, twy = ty * w, twz = tz * w, txx = tx * x, txy = ty * x, txz = tz * x, tyy = ty * y, tyz = tz * y, tzz = tz * z;
+		const float r[9] = {1.f - (tyy + tzz), txy + twz, txz - twy,   // column 0
+		                    txy - twz, 1.f - (txx + tzz), tyz + twx,   // column 1
+		                    txz + twy, tyz - twx, 1.f - (txx + tyy)};  // column 2
+		for (int i = 0; i < 9; ++i) out[i] = r[i];
+		for (int i = 0; i < 3; ++i) out[9 + i] = T[i];
+	}
+	// CameraKeyframe(Matrix<float, 3, 4>, ...): Quaternionf(Matrix3f) (the trace and largest-diagonal branches); m column-major
+	static CameraKeyframe from_matrix(const float m[12], float sl, float sc, float fv, float df) {
+		CameraKeyframe k;
+		auto at = [&](int r, int c) { return m[c * 3 + r]; };
+		float t = (at(0, 0) + at(1, 1)) + at(2, 2);
+		if (t > 0.f) {
+			t = std::sqrt(t + 1.f);
+			k.R[3] = 0.5f * t;
+			t = 0.5f / t;
+			k.R[0] = (at(2, 1) - at(1, 2)) * t;
+			k.R[1] = (at(0, 2) - at(2, 0)) * t;
+			k.R[2] = (at(1, 0) - at(0, 1)) * t;
+		} else {
+			int i = 0;
+			if (at(1, 1) > at(0, 0)) i = 1;
+			if (at(2, 2) > at(i, i)) i = 2;
+			const int j = (i + 1) % 3, l = (j + 1) % 3;
+			t = std::sqrt(at(i, i) - at(j, j) - at(l, l) + 1.f);
+			k.R[i] = 0.5f * t;
+			t = 0.5f / t;
+			k.R[3] = (at(l, j) - at(j, l)) * t;
+			k.R[j] = (at(j, i) + at(i, j)) * t;
+			k.R[l] = (at(l, i) + at(i, l)) * t;
+		}
+		for (int a = 0; a < 3; ++a) k.T[a] = m[9 + a];
+		k.slice = sl; k.scale = sc; k.fov = fv; k.dof = df;
+		return k;
+	}
+	CameraKeyframe operator*(float f) const {
+		CameraKeyframe k;
+		for (int i = 0; i < 4; ++i) k.R[i] = R[i] * f;
+		for (int i = 0; i < 3; ++i) k.T[i] = T[i] * f;
+		k.slice = slice * f; k.scale = scale * f; k.fov = fov * f; k.dof = dof * f;
+		return k;
+	}
+	CameraKeyframe operator+(const CameraKeyframe& rhs) const {  // the short path: flip rhs's quaternion when the dot product is negative
+		const float s = dot4(rhs.R, R) < 0.f ? -1.f : 1.f;
+		CameraKeyframe k;
+		for (int i = 0; i < 4; ++i) k.R[i] = R[i] + s * rhs.R[i];
+		for (int i = 0; i < 3; ++i) k.T[i] = T[i] + rhs.T[i];
+		k.slice = slice + rhs.slice; k.scale = scale + rhs.scale; k.fov = fov + rhs.fov; k.dof = dof + rhs.dof;
+		return k;
+	}
+};
+
+// spline (camera_path.cu:52-70): the cubic B-spline branch the reference compiles (its Catmull-Rom branch is `if (0)`)
+inline CameraKeyframe spline(float t, const CameraKeyframe& p0, const CameraKeyframe& p1, const CameraKeyframe& p2, const CameraKeyframe& p3) {
+	const float tt = t * t, ttt = t * t * t;
+	const float a = (1 - t) * (1 - t) * (1 - t) * (1.f / 6.f);
+	const float b = (3.f * ttt - 6.f * tt + 4.f) * (1.f / 6.f);
+	const float c = (-3.f * ttt + 3.f * tt + 3.f * t + 1.f) * (1.f / 6.f);
+	const float d = ttt * (1.f / 6.f);
+	return p0 * a + p1 * b + p2 * c + p3 * d;
+}
+
+struct CameraPath {
+	std::vector<CameraKeyframe> m_keyframes;
+	float m_playtime = 0.f;
+	const CameraKeyframe& get_keyframe(int i) const { return m_keyframes[(size_t)std::min(std::max(i, 0), (int)m_keyframes.size() - 1)]; }
+	CameraKeyframe eval_camera_path(float t) const {
+		if (m_keyframes.empty()) return {};
+		t *= (float)(m_keyframes.size() - 1);
+		const int t1 = (int)std::floor(t);
+		return spline(t - std::floor(t), get_keyframe(t1 - 1), get_keyframe(t1), get_keyframe(t1 + 1), get_keyframe(t1 + 2));
+	}
+};
+
 // Testbed::marching_cubes (testbed_nerf.cu:4614-4649): density on the grid, marching cubes, normals and colours. The mesh stays in the
 // context; the return value is the triangle count, like the reference's. density_dev: caller scratch of res[0]*res[1]*res[2] floats
 // (res rounded up to multiples of 16 here, as the reference does); NULL meshes an existing grid given as grid_dev instead
@@ -258,6 +353,15 @@ inline RgbaPng rgba_png(Context& ctx, const float* rgba_dev, const int32_t res[3
 	check(nsb_rgba_png(ctx.get(), rgba_dev, res, swap_y_z ? 1 : 0, static_cast<uint8_t*>(px.get()), stream), "nsb_rgba_png");
 	detail::download(p.pixels.data(), px.get(), p.pixels.size(), stream);
 	return p;
+}
+// Testbed::render_to_cpu (python_api.cu:129-175) once its sub-frames are known: every sub-frame rendered and accumulated, one tonemap, the
+// float4 frame copied to rgba_host (width * height * 4 floats) and the stream synchronised. accumulate_dev / out_rgba_dev: caller device
+// buffers of the frame's size (the reference's m_windowless_render_surface).
+inline void render_to_cpu(Context& ctx, const std::vector<NsbFrame>& sub_frames, const NsbTonemap& tm, float* accumulate_dev, float* out_rgba_dev,
+                          float* rgba_host, void* stream) {
+	if (sub_frames.empty()) throw std::runtime_error("render_to_cpu: no sub-frames");
+	check(nsb_render_accumulate(ctx.get(), sub_frames.data(), (uint32_t)sub_frames.size(), &tm, accumulate_dev, out_rgba_dev, stream), "nsb_render_accumulate");
+	detail::download(rgba_host, out_rgba_dev, (size_t)sub_frames[0].width * sub_frames[0].height * 16, stream);
 }
 #endif  // NSB_HOST_HAVE_CUDART
 

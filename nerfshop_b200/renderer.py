@@ -9,6 +9,8 @@
       nerfshop_b200.mesh builds the reference's Python-facing calls on them
   NerfRenderer.rgba_on_grid / density_png / rgba_png <- Testbed::get_rgba_on_grid (testbed_nerf.cu:4588-4612) and the pixel loops of
       save_density_grid_to_png / save_rgba_grid_to_png_sequence (marching_cubes.cu:898-1015); nerfshop_b200.slices writes the files
+  NerfRenderer.render_accumulate / frame_to_rgba8 <- Testbed::render_to_cpu's sub-frame loop (python_api.cu:129-175) and scripts/run.py's
+      8-bit video frames (write_image, scripts/common.py:122-178); nerfshop_b200.camera_path builds camera paths and videos on them
 
 torch is used for device memory and streams only; every computation is a call into libnerfshop_b200.so.
 """
@@ -269,6 +271,38 @@ class NerfRenderer:
             out = torch.empty_like(accumulate_buffer)
         abi.check(self.lib, self.lib.nsb_tonemap(self.ctx, accumulate_buffer.data_ptr(), out.data_ptr(), W, H, C.byref(params),
                                                  torch.cuda.current_stream().cuda_stream), "nsb_tonemap")
+        return out
+
+    # ---- whole output frames (Testbed::render_to_cpu's sub-frame loop, scripts/run.py's 8-bit frames) ------------------------------
+    def render_accumulate(self, frames, tonemap: "abi.NsbTonemap", accumulate=None, out=None, stream=None):
+        """nsb_render_accumulate: every sub-frame rendered and accumulated (spp = its spp_index), then one tonemap. frames: NsbFrames of one
+        size; accumulate / out: float32 CUDA tensors [H, W, 4] (allocated if None). Returns (accumulate, out). Stream-ordered."""
+        torch = _torch()
+        frames = list(frames)
+        if not frames:
+            raise ValueError("render_accumulate: no sub-frames")
+        H, W = frames[0].height, frames[0].width
+        dev = torch.device("cuda", self.device)
+        if accumulate is None:
+            accumulate = torch.empty((H, W, 4), dtype=torch.float32, device=dev)
+        if out is None:
+            out = torch.empty((H, W, 4), dtype=torch.float32, device=dev)
+        arr = (abi.NsbFrame * len(frames))(*frames)
+        s = torch.cuda.current_stream(dev).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_render_accumulate(self.ctx, arr, len(frames), C.byref(tonemap), accumulate.data_ptr(), out.data_ptr(), s),
+                  "nsb_render_accumulate")
+        return accumulate, out
+
+    def frame_to_rgba8(self, rgba, exposure: float = 0.0, n_channels: int = 4, out=None, stream=None):
+        """nsb_frame_to_rgba8 on a float32 CUDA tensor [H, W, 4] of linear premultiplied RGBA: run.py's np.clip(frame * 2**exposure, 0, 1)
+        and write_image's 8-bit pixels, uint8 CUDA tensor [H, W, n_channels] (3: RGB without alpha). Stream-ordered."""
+        torch = _torch()
+        H, W = rgba.shape[0], rgba.shape[1]
+        if out is None:
+            out = torch.empty((H, W, n_channels), dtype=torch.uint8, device=torch.device("cuda", self.device))
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_frame_to_rgba8(self.ctx, rgba.data_ptr(), W, H, float(exposure), int(n_channels), out.data_ptr(), s),
+                  "nsb_frame_to_rgba8")
         return out
 
     # ---- operator-level entry points ---------------------------------------------------------------------
