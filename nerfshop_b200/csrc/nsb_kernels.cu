@@ -2339,7 +2339,8 @@ extern "C" NsbStatus nsb_mesh_optimise(NsbContext* c, const NsbMeshOptimise* p, 
 	if (!c->has_model) return fail(NSB_ERR_STATE, "nsb_mesh_optimise: nsb_upload_model has not been called");
 	if (!c->has_mesh) return fail(NSB_ERR_STATE, "nsb_mesh_optimise: no mesh (nsb_marching_cubes)");
 	const uint32_t nv = (uint32_t)c->mesh_nv, rows = (uint32_t)((c->mesh_nv + 127ull) & ~127ull);
-	if (rows == 0 || n_steps == 0) return NSB_OK;
+	if (rows == 0) { c->mesh_normals_ok = true; return NSB_OK; }  // an empty mesh has no normals to compute, as in nsb_mesh_shade
+	if (n_steps == 0) return NSB_OK;
 	CU(cudaSetDevice(c->device));
 	cudaStream_t st = (cudaStream_t)stream_;
 	const NsbStatus csr = mesh_build_csr(c, st);

@@ -190,7 +190,10 @@ int orc_mesh_opt_gradient(uint32_t n_rows, const float* pos, const uint32_t* ind
 		const V3 sg = v3(fmaf(-inv, sum[v].x, src.x), fmaf(-inv, sum[v].y, src.y), fmaf(-inv, sum[v].z, src.z));
 		const V3 n = normalized3(v3(grad[3 * v], grad[3 * v + 1], grad[3 * v + 2]));
 		const V3 nn = normalized3(nrm[v]);
-		const float sgn = copysignf(1.0f, h2f(dens[v]) - k[0]);
+		// the sign of dens - thresh as the device takes it: a NaN difference is the GPU's canonical NaN, whose sign bit is clear, so it counts
+		// as +1 whatever the signs of its NaN operands (the host's subtraction would pass a -NaN threshold's sign through)
+		const float d = h2f(dens[v]) - k[0];
+		const float sgn = std::isnan(d) ? 1.0f : copysignf(1.0f, d);
 		if (grad_out) {
 			grad_out[3 * v] = fmaf(-nn.x, k[3], fmaf(n.x * sgn, k[2], sg.x * k[1]));
 			grad_out[3 * v + 1] = fmaf(-nn.y, k[3], fmaf(n.y * sgn, k[2], sg.y * k[1]));
@@ -203,7 +206,9 @@ int orc_mesh_opt_gradient(uint32_t n_rows, const float* pos, const uint32_t* ind
 // tcnn Adam (learning rate 1e-4, beta1 0.9, beta2 0.99, epsilon 1e-8) on n coordinates, each a non-matrix parameter: skipped while its gradient
 // is 0, its own step counter. Published adam_step: effective_learning_rate = lr_t / (sqrtf(v) + epsilon), new = weight - effective_learning_rate * m,
 // with the moment updates and the subtraction contracted as nvcc does. m1, m2, steps: in/out.
-int orc_adam_step(uint32_t n, const float* x_in, const float* g, float* m1, float* m2, uint32_t* steps, float* x_out) {
+// pows (may be NULL): [n_pows x 2] floats, row t = {powf(0.9f, t), powf(0.99f, t)} as the device computes them (tcnn runs powf on the GPU;
+// the host's powf is not correctly rounded and need not agree with it). NULL: the host's powf. Returns 2 when a step count reaches n_pows.
+int orc_adam_step(uint32_t n, const float* x_in, const float* g, float* m1, float* m2, uint32_t* steps, float* x_out, const float* pows, uint32_t n_pows) {
 	const float B1 = 0.9f, B2 = 0.99f, LR = 1e-4f, EPS = 1e-8f;
 	for (uint32_t j = 0; j < n; ++j) {
 		float x = x_in[j];
@@ -211,7 +216,9 @@ int orc_adam_step(uint32_t n, const float* x_in, const float* g, float* m1, floa
 			m1[j] = fmaf(B1, m1[j], (1.0f - B1) * g[j]);
 			m2[j] = fmaf(B2, m2[j], (1.0f - B2) * (g[j] * g[j]));
 			const uint32_t t = ++steps[j];
-			const float lr = LR * (sqrtf(1.0f - powf(B2, (float)t)) / (1.0f - powf(B1, (float)t)));
+			if (pows && t >= n_pows) return 2;
+			const float p1 = pows ? pows[2 * (size_t)t] : powf(B1, (float)t), p2 = pows ? pows[2 * (size_t)t + 1] : powf(B2, (float)t);
+			const float lr = LR * (sqrtf(1.0f - p2) / (1.0f - p1));
 			const float eff = lr / (sqrtf(m2[j]) + EPS);
 			x = fmaf(-eff, m1[j], x);
 		}
@@ -222,10 +229,10 @@ int orc_adam_step(uint32_t n, const float* x_in, const float* g, float* m1, floa
 
 // One step of Testbed::optimise_mesh_step after the network: orc_mesh_opt_gradient, then orc_adam_step on every coordinate of the n_rows rows.
 int orc_mesh_opt_step(uint32_t n_rows, const float* pos, const uint32_t* indices, uint32_t n_tris, const uint16_t* dens, const float* grad, const float* k,
-                      float* m1, float* m2, uint32_t* steps, float* pos_out, float* normals) {
+                      float* m1, float* m2, uint32_t* steps, float* pos_out, float* normals, const float* pows, uint32_t n_pows) {
 	std::vector<float> g(3 * (size_t)n_rows);
 	orc_mesh_opt_gradient(n_rows, pos, indices, n_tris, dens, grad, k, nullptr, normals, g.data());
-	return orc_adam_step(3 * n_rows, pos, g.data(), m1, m2, steps, pos_out);
+	return orc_adam_step(3 * n_rows, pos, g.data(), m1, m2, steps, pos_out, pows, n_pows);
 }
 
 }  // extern "C"

@@ -41,9 +41,9 @@ def lib() -> C.CDLL:
         vp = C.c_void_p
         l.orc_density_gradient.argtypes = [C.POINTER(orc.OrcScene), vp, C.c_uint32, vp, vp, vp, vp]
         l.orc_density_f64.argtypes = [C.POINTER(orc.OrcScene), vp, C.c_uint32, vp, vp]
-        l.orc_mesh_opt_step.argtypes = [C.c_uint32, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp]
+        l.orc_mesh_opt_step.argtypes = [C.c_uint32, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32]
         l.orc_mesh_opt_gradient.argtypes = [C.c_uint32, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp]
-        l.orc_adam_step.argtypes = [C.c_uint32, vp, vp, vp, vp, vp, vp]
+        l.orc_adam_step.argtypes = [C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint32]
         l.orc_set_mlp_policy.argtypes = [C.c_int]
         _lib = l
     return _lib
@@ -81,8 +81,18 @@ def density_f64(o: "orc.Oracle", pos: np.ndarray, want_grad: bool = True):
     return dens, grad
 
 
-def mesh_opt_step(pos, faces, dens_fp16, grad, thresh, smooth_amount, density_amount, inflate_amount, state=None):
+def _pows(pows):
+    """(pointer, row count) of a debiasing powers table [n, 2] float32 (row t = powf(0.9f, t), powf(0.99f, t)); (None, 0) for the host's powf."""
+    if pows is None:
+        return None, 0, None
+    p = np.ascontiguousarray(pows, np.float32)
+    assert p.ndim == 2 and p.shape[1] == 2
+    return _ptr(p), p.shape[0], p
+
+
+def mesh_opt_step(pos, faces, dens_fp16, grad, thresh, smooth_amount, density_amount, inflate_amount, state=None, pows=None):
     """One step on all rows of pos [rows, 3] float32. state = (m1, m2, steps) arrays [rows, 3] (zeros when None), updated in place.
+    pows: Adam's debiasing powers [n, 2] (row t = powf(0.9f, t), powf(0.99f, t)), the host's powf when None.
     Returns (new positions, normals of `pos`, state)."""
     pos = np.ascontiguousarray(pos, np.float32)
     rows = pos.shape[0]
@@ -93,8 +103,9 @@ def mesh_opt_step(pos, faces, dens_fp16, grad, thresh, smooth_amount, density_am
     out, nrm = np.zeros_like(pos), np.zeros_like(pos)
     d = np.ascontiguousarray(dens_fp16, np.uint16)
     g = np.ascontiguousarray(grad, np.float32)
+    pp, npw, _keep = _pows(pows)
     assert lib().orc_mesh_opt_step(rows, _ptr(pos), _ptr(F), F.size // 3, _ptr(d), _ptr(g), _ptr(k), _ptr(state[0]), _ptr(state[1]), _ptr(state[2]),
-                                   _ptr(out), _ptr(nrm)) == 0
+                                   _ptr(out), _ptr(nrm), pp, npw) == 0
     return out, nrm, state
 
 
@@ -110,12 +121,14 @@ def mesh_opt_gradient(pos, faces, dens_fp16, grad, thresh, smooth_amount, densit
     return sums, nrm, g
 
 
-def adam_step(x, g, state=None):
-    """The restated tcnn Adam on the coordinates of x [rows, 3] with gradient g; state = (m1, m2, steps), zeros when None, updated in place."""
+def adam_step(x, g, state=None, pows=None):
+    """The restated tcnn Adam on the coordinates of x [rows, 3] with gradient g; state = (m1, m2, steps), zeros when None, updated in place.
+    pows: as mesh_opt_step's."""
     x = np.ascontiguousarray(x, np.float32)
     g = np.ascontiguousarray(g, np.float32)
     if state is None:
         state = (np.zeros(x.shape, np.float32), np.zeros(x.shape, np.float32), np.zeros(x.shape, np.uint32))
     out = np.zeros_like(x)
-    assert lib().orc_adam_step(x.size, _ptr(x), _ptr(g), _ptr(state[0]), _ptr(state[1]), _ptr(state[2]), _ptr(out)) == 0
+    pp, npw, _keep = _pows(pows)
+    assert lib().orc_adam_step(x.size, _ptr(x), _ptr(g), _ptr(state[0]), _ptr(state[1]), _ptr(state[2]), _ptr(out), pp, npw) == 0
     return out, state

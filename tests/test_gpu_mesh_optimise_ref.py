@@ -74,13 +74,22 @@ def test_one_step_vs_reference(mr):
     P_ref, _ = mo.adam_step(V0[rows], g_ref)
     V0r = V0[rows]
 
+    agree_with_reference(rows, nv, V1, P_ref, g_our, g_ref, s_our, s_ref, n_our, n_ref, min_agree=0.3)
+    # the step moved the mesh as the reference's would: by about lr per coordinate with a non-zero gradient
+    moved = np.abs(V1 - V0r)
+    assert (moved <= 1.01e-4).all() and (moved > 0).mean() > 0.9
+
+
+def agree_with_reference(rows, nv, V1, P_ref, g_our, g_ref, s_our, s_ref, n_our, n_ref, min_agree):
+    """The agreement rule on the compared rows: bit for bit where the reference's atomic 1-ring sums and normals equal this repository's
+    (and on the padding rows, which have no triangles), the documented tolerance elsewhere. Returns the share of rows whose sums agree."""
     agree = (s_ref.view(np.uint32) == s_our.view(np.uint32)).all(1) & (n_ref.view(np.uint32) == n_our.view(np.uint32)).all(1)
     padding = rows >= nv
-    print(f"\n{rows.size} rows compared ({nv} vertices, {V0.shape[0]} rows): 1-ring sums and normals bit-equal on {100 * agree.mean():.2f} %; "
+    print(f"\n{rows.size} rows compared ({nv} vertices): 1-ring sums and normals bit-equal on {100 * agree.mean():.2f} %; "
           f"positions bit-equal on {100 * (V1 == P_ref).all(1).mean():.2f} %")
     # the atomics reorder the sums of most vertices with more than a few triangles (measured: 42 % of the rows agree bit for bit); the
     # bit-exact check below covers those rows and the padding, which have no triangles
-    assert agree.mean() > 0.3 and agree[padding].all()
+    assert agree.mean() > min_agree and agree[padding].all()
     # where the atomic sums agree: the reference's opt gradient and the moved positions, bit for bit (padding rows included)
     np.testing.assert_array_equal(g_our[agree].view(np.uint32), g_ref[agree].view(np.uint32))
     np.testing.assert_array_equal(V1[agree].view(np.uint32), P_ref[agree].view(np.uint32))
@@ -91,11 +100,13 @@ def test_one_step_vs_reference(mr):
     print(f"rows whose sums differ: {rest.sum()}; opt gradient relative difference max {rel[same_sign].max() if same_sign.any() else 0:.2e}; "
           f"coordinates with a sign change: {(~same_sign).sum()}")
     assert (~same_sign).sum() <= max(2, int(1e-3 * same_sign.size))
-    # one rounding of the new position, plus a few ulps of the step lr * m / (sqrt(v) + eps) itself, which show where the position is near 0
-    tol = np.spacing(np.maximum(np.abs(V1[rest]), np.abs(P_ref[rest])).astype(np.float32)) + 4 * np.spacing(np.float32(1e-4))
+    # one rounding of the new position, plus a few ulps of the step lr * m / (sqrt(v) + eps) itself, which show where the position is near 0,
+    # plus the change of that first step, lr * g / (|g| + 10 eps), with the gradient: lr * 10 eps * |dg| / (|g| + 10 eps)^2, which only matters
+    # where |g| is near 10 eps = 1e-7 (a smoothing gradient that nearly cancels)
+    g_min = np.minimum(np.abs(g_our[rest]), np.abs(g_ref[rest])).astype(np.float64)
+    dstep = 1.01e-4 * 1e-7 * np.abs(g_our[rest].astype(np.float64) - g_ref[rest]) / (g_min + 1e-7) ** 2
+    tol = np.spacing(np.maximum(np.abs(V1[rest]), np.abs(P_ref[rest])).astype(np.float32)) + 4 * np.spacing(np.float32(1e-4)) + dstep
     off = np.abs(V1[rest] - P_ref[rest])
-    print(f"positions that differ: {(off > 0).sum()} coordinates, at most {(off / tol)[same_sign].max():.2f} of the tolerance")
+    print(f"positions that differ: {(off > 0).sum()} coordinates, at most {(off / tol)[same_sign].max() if same_sign.any() else 0:.2f} of the tolerance")
     assert (off[same_sign] <= tol[same_sign]).all()
-    # the step moved the mesh as the reference's would: by about lr per coordinate with a non-zero gradient
-    moved = np.abs(V1 - V0r)
-    assert (moved <= 1.01e-4).all() and (moved > 0).mean() > 0.9
+    return agree.mean()
