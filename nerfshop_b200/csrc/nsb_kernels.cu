@@ -866,14 +866,17 @@ __device__ __forceinline__ void tonemap_curve(float* x, int curve) {  // render_
 		const float white_scale = denom / nom;
 		k0 = 4.0f * k0 * white_scale; k1 = 2.0f * k1 * white_scale; k2 = k2 * white_scale; k3 = 4.0f * k3; k4 = 2.0f * k4;
 	} else {  // Reinhard
-		float Y = 0.2126f * x[0] + 0.7152f * x[1] + 0.0722f * x[2];
+		// luminance_coefficients.dot(x): Eigen reduces a 3-vector as x0 + (x1 + x2), which nvcc contracts into these two FMAs
+		float Y = __fmaf_rn(0.2126f, x[0], __fmaf_rn(0.7152f, x[1], __fmul_rn(0.0722f, x[2])));
 		float s = 1.0f / (Y + 1.0f);
 		for (int k = 0; k < 3; ++k) x[k] *= s;
 		return;
 	}
-	for (int k = 0; k < 3; ++k) {
-		float sq = x[k] * x[k];
-		x[k] = (sq * k0 + k1 * x[k] + k2) / (k3 * sq + k4 * x[k] + k5);
+	for (int k = 0; k < 3; ++k) {  // color_sq * k0 + k1 * x + k2 and k3 * color_sq + k4 * x + k5 as nvcc contracts them in the reference
+		const float sq = __fmul_rn(x[k], x[k]);
+		const float nom = __fadd_rn(__fmaf_rn(sq, k0, __fmul_rn(k1, x[k])), k2);
+		const float denom = __fadd_rn(__fmaf_rn(k3, sq, __fmul_rn(k4, x[k])), k5);
+		x[k] = nom / denom;
 	}
 }
 __global__ void k_tonemap(int n, const float4* __restrict__ acc, float4* __restrict__ out, NsbTonemap p) {

@@ -1318,7 +1318,7 @@ int orc_tonemap(const float* acc, float* out, int n, const NsbTonemap* p) {
 		if (p->tonemap_curve != NSB_TONEMAP_IDENTITY) {
 			for (int k = 0; k < 3; ++k) c[k] = fmaxf(c[k], 0.0f);
 			if (p->tonemap_curve == NSB_TONEMAP_REINHARD) {
-				float Y = 0.2126f * c[0] + 0.7152f * c[1] + 0.0722f * c[2];
+				float Y = 0.2126f * c[0] + (0.7152f * c[1] + 0.0722f * c[2]);  // luminance_coefficients.dot(x): Eigen's x0 + (x1 + x2)
 				for (int k = 0; k < 3; ++k) c[k] *= 1.0f / (Y + 1.0f);
 			} else {
 				float k0, k1, k2, k3, k4, k5;

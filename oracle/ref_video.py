@@ -27,8 +27,16 @@ def lib() -> C.CDLL:
         l.refcu_destroy.restype = None
         l.refvid_render_to_cpu.argtypes = [V, C.POINTER(abi.NsbFrame), C.c_int, V, V, C.c_float, C.POINTER(C.c_float), C.c_int, C.c_int, C.c_int, C.c_int,
                                            V, V, V, V]
+        if hasattr(l, "refvid_postprocess"):  # a prebuilt library from before the entry point lacks it (serves_postprocess)
+            l.refvid_postprocess.argtypes = [V, C.c_int, C.c_uint32, C.c_int, C.c_int, C.c_int, V, V, C.POINTER(C.c_float), C.c_int, V]
         _lib = l
     return _lib
+
+
+def serves_postprocess() -> bool:
+    """The library exists and has refvid_postprocess. A prebuilt one older than that entry point does not: the tests then replay the
+    reference's stored results, as tests/ref_golden.py does for oracle/ref.py's later entry points."""
+    return ref_video_build.build() is not None and hasattr(lib(), "refvid_postprocess")
 
 
 def render_to_cpu(bitfield, ops, frames, renderer, tm: abi.NsbTonemap) -> np.ndarray:
@@ -60,3 +68,37 @@ def render_to_cpu(bitfield, ops, frames, renderer, tm: abi.NsbTonemap) -> np.nda
         return out.cpu().numpy()
     finally:
         l.refcu_destroy(h)
+
+
+def tonemap_rows(tms) -> np.ndarray:
+    """NsbTonemaps -> the [n, 9] float32 rows refvid_postprocess reads (colour space aside, which the accumulation fixes)."""
+    return np.array([[t.exposure, *t.background_color, t.output_color_space, t.tonemap_curve, t.clamp_output_color, 0.0] for t in tms], np.float32)
+
+
+def postprocess(frames, spp0: int, color_space: int, acc0=None, tm_rows=None):
+    """The reference's accumulate_kernel and tonemap_kernel on caller buffers, launched as CudaRenderBuffer does (16x8 blocks).
+
+    frames: float32 [n, H, W, 4] accumulated in order with sample counts spp0, spp0 + 1, ... (the accumulation is zeroed when the count is
+    0, else it starts from acc0 [H, W, 4]); n may be 0 to tonemap acc0 itself. tm_rows: tonemap_rows(...) or None.
+    Returns (the accumulation after every call [H*W, n, 4], every tonemapped surface [H*W, n_tm, 4] or None): pixel-major, so a stored
+    row sample keeps whole pixels."""
+    import torch
+
+    l = lib()
+    frames = np.ascontiguousarray(frames, np.float32)
+    n, H, W = frames.shape[0], frames.shape[1], frames.shape[2]
+    if acc0 is not None:
+        H, W = acc0.shape[0], acc0.shape[1]
+    px = H * W
+    f_dev = torch.from_numpy(frames).cuda() if n else None
+    acc = torch.from_numpy(np.ascontiguousarray(acc0, np.float32)).cuda() if acc0 is not None else torch.zeros((H, W, 4), dtype=torch.float32, device="cuda")
+    hist = torch.empty((max(n, 1), px, 4), dtype=torch.float32, device="cuda")
+    rows = None if tm_rows is None else np.ascontiguousarray(tm_rows, np.float32)
+    n_tm = 0 if rows is None else rows.shape[0]
+    out = torch.empty((max(n_tm, 1), px, 4), dtype=torch.float32, device="cuda")
+    torch.cuda.synchronize()
+    rc = l.refvid_postprocess(f_dev.data_ptr() if n else None, n, spp0, W, H, color_space, acc.data_ptr(), hist.data_ptr() if n else None,
+                              rows.ctypes.data_as(C.POINTER(C.c_float)) if n_tm else None, n_tm, out.data_ptr() if n_tm else None)
+    assert rc == 0
+    hist = hist[:n].permute(1, 0, 2).contiguous().cpu().numpy() if n else None
+    return hist, (out.permute(1, 0, 2).contiguous().cpu().numpy() if n_tm else None)

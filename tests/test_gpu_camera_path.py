@@ -324,13 +324,24 @@ def _ref_video_available():
     return ref_video_build.build() is not None
 
 
+# tonemaps other than render_frame's default: (curve, input colour space, output colour space, clamp, exposure)
+_TONEMAPS = {
+    "reinhard_srgb_clamp": (abi.NSB_TONEMAP_REINHARD, abi.NSB_COLOR_LINEAR, abi.NSB_COLOR_SRGB, 1, 0.0),
+    "aces_exposure": (abi.NSB_TONEMAP_ACES, abi.NSB_COLOR_LINEAR, abi.NSB_COLOR_LINEAR, 0, 1.3),
+    "hable_srgb_accumulate": (abi.NSB_TONEMAP_HABLE, abi.NSB_COLOR_SRGB, abi.NSB_COLOR_SRGB, 0, 0.0),
+    "visposneg": (abi.NSB_TONEMAP_IDENTITY, abi.NSB_COLOR_VISPOSNEG, abi.NSB_COLOR_LINEAR, 0, -0.5),
+}
+
+
 @pytest.mark.skipif(not (_ref_video_available() or os.path.isdir(os.path.join(os.path.dirname(__file__), "golden", "ref", "test_gpu_camera_path"))),
                     reason="neither oracle/_ref nor stored reference results (tests/golden/ref/)")
-@pytest.mark.parametrize("edits", [False, True], ids=["plain", "e1"])
-def test_render_accumulate_vs_reference_cuda(scene, renderer, edits):
+@pytest.mark.parametrize("edits, tonemap", [(False, None), (True, None)] + [(False, k) for k in _TONEMAPS] + [(True, "reinhard_srgb_clamp")],
+                         ids=["plain", "e1"] + [f"plain_{k}" for k in _TONEMAPS] + ["e1_reinhard_srgb_clamp"])
+def test_render_accumulate_vs_reference_cuda(scene, renderer, edits, tonemap):
     """The same sub-frame cameras through the reference's clear_frame -> render_nerf -> accumulate_kernel -> tonemap_kernel, once per
     sub-frame as render_frame runs them (oracle/ref_video_driver_cuda.cu): L-inf 0 without edits (as the frame-domain tests), <= 1e-3 with
-    E1 (DESIGN §6). Where oracle/_ref is absent the stored results of the reference are replayed."""
+    E1 (DESIGN §6), under render_frame's default tonemap and under every curve, sRGB accumulation and output, clamping, exposure and
+    VisPosNeg. Where oracle/_ref is absent the stored results of the reference are replayed."""
     import ref_golden
 
     from oracle import ref_video
@@ -340,17 +351,22 @@ def test_render_accumulate_vs_reference_cuda(scene, renderer, edits):
     frames = _sub_frames(base, 8)
     tm = _tonemap()
     tm.background_color[:] = [0.1, 0.2, 0.3, 0.5]
+    digest = []
+    if tonemap is not None:
+        tm.tonemap_curve, tm.color_space, tm.output_color_space, tm.clamp_output_color, tm.exposure = _TONEMAPS[tonemap]
+        digest = [np.array(_TONEMAPS[tonemap], np.float32)]
     ops = [op.to_op() for op in fx.e1(model)] if edits else None
     cams = np.array([[list(f.camera0), list(f.camera1), list(f.focal_length) + [0.0] * 10] for f in frames], np.float32)  # the inputs' digest
     try:
         renderer.set_edit_operators(ops or [])
-        want = ref_golden._call(_ref_video_available(), lambda c: ref_video.render_to_cpu(occ, ops, frames, renderer, tm), cams)
+        want = ref_golden._call(_ref_video_available(), lambda c, *_: ref_video.render_to_cpu(occ, ops, frames, renderer, tm), cams, *digest)
         _, got = renderer.render_accumulate(frames, tm)
         got = got.cpu().numpy()
     finally:
         renderer.reset_edit_operators()
     got, want = ref_golden.ref.match(got, want)
     err = float(np.abs(got - want).max())
-    print(f"\nrender_accumulate vs the reference's render_frame sequence ({'E1' if edits else 'plain'}, 8 sub-frames): L-inf {err:.3e}")
+    print(f"\nrender_accumulate vs the reference's render_frame sequence ({'E1' if edits else 'plain'}, {tonemap or 'default tonemap'}, 8 sub-frames): "
+          f"L-inf {err:.3e}")
     assert float(want[..., 3].mean()) > 0.05
     assert err <= (1e-3 if edits else 0.0)
