@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define NSB_ABI_VERSION 8
+#define NSB_ABI_VERSION 9
 
 /* reference: common_nerf.h:16-39 */
 #define NSB_NERF_GRIDSIZE 128u
@@ -539,6 +539,27 @@ NsbStatus nsb_render_accumulate(NsbContext* ctx, const NsbFrame* frames, uint32_
  * powf is CUDA's: a byte may differ from numpy's by one where the float lies within an ulp of a quantisation boundary. Stream-ordered. */
 NsbStatus nsb_frame_to_rgba8(NsbContext* ctx, const float* rgba_dev, int32_t w, int32_t h, float exposure, int32_t n_channels, uint8_t* out_dev,
                              void* stream);
+
+/* ---- image-quality metrics (ABI 9): scripts/run.py's --test_transforms block (run.py:215-302) ------------------------------------ */
+/* replaces read_image (scripts/common.py:147-161) after the decode, and run.py's sRGB blend (run.py:264-270), on DEVICE 8-bit pixels
+ * (w*h pixels of n_channels = 3 or 4 bytes, row-major): per pixel, in float32 with every operation rounded on its own, c = byte / 255,
+ * c = srgb_to_linear(c) on the colour (c > 0.04045 ? ((c + 0.055) / 1.055)^2.4 : c / 12.92), colour * alpha; RGB gets alpha 1.
+ * srgb_blend = 1 (RGBA only, run.py with the colour space sRGB): colour / alpha (0 where alpha is 0), linear_to_srgb, * alpha, then
+ * + (1 - alpha) * background on all four channels, srgb_to_linear on the colour. background: HOST float[4], read only with srgb_blend.
+ * pow is correctly rounded float32 (float64 pow, rounded once). out_rgba_dev: DEVICE float4[w*h], 16-byte aligned. Stream-ordered. */
+NsbStatus nsb_reference_image(NsbContext* ctx, const uint8_t* pixels_dev, int32_t w, int32_t h, int32_t n_channels, int32_t srgb_blend,
+                              const float background[4], float* out_rgba_dev, void* stream);
+/* replaces run.py's per-frame metric block (run.py:286-290) on two DEVICE float4[w*h] frames (16-byte aligned; linear premultiplied RGBA,
+ * e.g. nsb_render_accumulate's output and nsb_reference_image's): A = clip(linear_to_srgb(image.rgb), 0, 1) with compute_error_img's
+ * clean-up (non-finite -> 0, max(., 0)), R the same for ref without it; the MSE map ((d0^2 + d1^2) + d2^2) / 3 with non-finite terms 0, and
+ * SSIM's map (common.py:190-207: luminance, the separable 5-tap blur with scipy's 'reflect' boundary along y then x, p1 * p2, non-finite
+ * -> 0), then both means as np.mean computes them (numpy's pairwise float32 sum, float32(float64(sum) / n)). Every step after the pows is
+ * numpy's float32 arithmetic in numpy's order; pow is correctly rounded float32. out_mse_ssim_dev: DEVICE float[2] = (MSE, SSIM), written
+ * on the stream, so frames can queue without a host synchronisation. mse_map_dev / ssim_map_dev: DEVICE float[w*h] (row-major) or NULL;
+ * for a NULL map the context keeps a buffer (4 B per pixel) that is allocated on the first call at a size and only grows. w*h < 2^31.
+ * Stream-ordered, no host synchronisation except when that buffer grows. */
+NsbStatus nsb_image_metrics(NsbContext* ctx, const float* image_rgba_dev, const float* ref_rgba_dev, int32_t w, int32_t h, float* out_mse_ssim_dev,
+                            float* mse_map_dev, float* ssim_map_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libnerfshop_b200.so")
 
-NSB_ABI_VERSION = 8
+NSB_ABI_VERSION = 9
 NSB_MLP_ACC_F32, NSB_MLP_ACC_F16 = 0, 1
 NSB_NERF_GRIDSIZE = 128
 NSB_NERF_CASCADES = 5
@@ -152,6 +152,7 @@ EXPORTED_SYMBOLS = [
     "nsb_density_gradient", "nsb_mesh_optimise",
     "nsb_rgba_on_grid", "nsb_density_png_extent", "nsb_density_png", "nsb_rgba_png",
     "nsb_render_accumulate", "nsb_frame_to_rgba8",
+    "nsb_reference_image", "nsb_image_metrics",
 ]
 
 _lib = None
@@ -234,6 +235,8 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.nsb_rgba_png.argtypes = [vp, vp, C.POINTER(i32), i32, vp, vp]
     lib.nsb_render_accumulate.argtypes = [vp, C.POINTER(NsbFrame), u32, C.POINTER(NsbTonemap), vp, vp, vp]
     lib.nsb_frame_to_rgba8.argtypes = [vp, vp, i32, i32, f32, i32, vp, vp]
+    lib.nsb_reference_image.argtypes = [vp, vp, i32, i32, i32, i32, C.POINTER(f32), vp, vp]
+    lib.nsb_image_metrics.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp]
     for name in EXPORTED_SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("nsb_last_error", "nsb_abi_version"):

@@ -936,6 +936,7 @@ __global__ void k_unpack_gathered(const float4* __restrict__ gathered, const flo
 #include "nsb_mesh_opt.cuh"
 #include "nsb_slices.cuh"
 #include "nsb_video.cuh"
+#include "nsb_eval.cuh"
 
 // =====================================================================================================
 // host side: context, uploads, C ABI
@@ -1054,6 +1055,8 @@ struct NsbContext {
 	DevBuf<uint32_t> opt_steps;
 	DevBuf<__half> opt_dens;
 	bool opt_fresh = true;
+	// nsb_image_metrics: the MSE and SSIM maps when the caller keeps none (8 B per pixel, grows only) and the pairwise-sum tree of each
+	DevBuf<float> eval_maps, eval_heap;
 
 	~NsbContext() {  // the device arrays free themselves
 		for (cudaEvent_t e : {ev0, ev1, evm, render_done[0], render_done[1], copy_done[0], copy_done[1]}) if (e) cudaEventDestroy(e);
@@ -2054,6 +2057,51 @@ extern "C" NsbStatus nsb_frame_to_rgba8(NsbContext* c, const float* rgba, int32_
 	const uint32_t n = (uint32_t)W * (uint32_t)H;
 	const float scale = (float)std::pow(2.0, (double)exposure);  // run.py's 2**exposure: a Python float, rounded to float32 against the float32 frame
 	video::k_rgba8<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(n, reinterpret_cast<const float4*>(rgba), scale, n_channels, out);
+	CU(cudaGetLastError());
+	return NSB_OK;
+}
+
+// ---- image-quality metrics (ABI 9): run.py's --test_transforms block on the device ---------------------------------------
+extern "C" NsbStatus nsb_reference_image(NsbContext* c, const uint8_t* pixels, int32_t W, int32_t H, int32_t n_channels, int32_t srgb_blend,
+                                         const float background[4], float* out, void* stream) {
+	if (!c || !pixels || !out || W <= 0 || H <= 0) return fail(NSB_ERR_INVALID, "bad arguments");
+	if ((uint64_t)W * (uint64_t)H > 0xffffffffull) return fail(NSB_ERR_INVALID, "image %dx%d has more than 2^32 pixels", W, H);
+	if (n_channels != 3 && n_channels != 4) return fail(NSB_ERR_INVALID, "n_channels must be 3 or 4, not %d", n_channels);
+	if (srgb_blend != 0 && srgb_blend != 1) return fail(NSB_ERR_INVALID, "srgb_blend must be 0 or 1, not %d", srgb_blend);
+	if (srgb_blend && !background) return fail(NSB_ERR_INVALID, "the sRGB blend needs a background colour");
+	if (((uintptr_t)out & 15u) != 0) return fail(NSB_ERR_INVALID, "the float4 output must be 16-byte aligned");
+	CU(cudaSetDevice(c->device));
+	const uint32_t n = (uint32_t)W * (uint32_t)H;
+	const float4 bg = background ? make_float4(background[0], background[1], background[2], background[3]) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+	evalm::k_reference_image<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(n, pixels, n_channels, srgb_blend, bg, reinterpret_cast<float4*>(out));
+	CU(cudaGetLastError());
+	return NSB_OK;
+}
+
+extern "C" NsbStatus nsb_image_metrics(NsbContext* c, const float* image, const float* ref, int32_t W, int32_t H, float* out_mse_ssim, float* mse_map,
+                                       float* ssim_map, void* stream_) {
+	if (!c || !image || !ref || !out_mse_ssim || W <= 0 || H <= 0) return fail(NSB_ERR_INVALID, "bad arguments");
+	if ((uint64_t)W * (uint64_t)H > 0x7fffffffull) return fail(NSB_ERR_INVALID, "image %dx%d has 2^31 pixels or more", W, H);
+	if (((uintptr_t)image & 15u) != 0 || ((uintptr_t)ref & 15u) != 0) return fail(NSB_ERR_INVALID, "the float4 images must be 16-byte aligned");
+	for (const float* p : {(const float*)out_mse_ssim, (const float*)mse_map, (const float*)ssim_map})
+		if (((uintptr_t)p & 3u) != 0) return fail(NSB_ERR_INVALID, "float outputs must be 4-byte aligned");
+	CU(cudaSetDevice(c->device));
+	cudaStream_t stream = (cudaStream_t)stream_;
+	const size_t n = (size_t)W * (size_t)H;
+	const size_t n_maps = (mse_map ? 0 : n) + (ssim_map ? 0 : n), n_heap = 2 * (2u << evalm::kDepth);
+	if (c->eval_maps.capacity() < n_maps || c->eval_heap.capacity() < n_heap) {  // grows only; the old buffers may still be read on `stream`
+		CU(cudaStreamSynchronize(stream));
+		CU(c->eval_maps.reserve(n_maps));
+		CU(c->eval_heap.reserve(n_heap));
+	}
+	float* m0 = mse_map ? mse_map : c->eval_maps.get();
+	float* m1 = ssim_map ? ssim_map : c->eval_maps.get() + (mse_map ? 0 : n);
+	const dim3 tiles((W + evalm::kTX - 1) / evalm::kTX, (H + evalm::kTY - 1) / evalm::kTY);
+	evalm::k_image_metrics<<<tiles, evalm::kThreads, 0, stream>>>(W, H, reinterpret_cast<const float4*>(image), reinterpret_cast<const float4*>(ref), m0, m1);
+	CU(cudaGetLastError());
+	evalm::k_pairwise_nodes<<<dim3((1u << evalm::kDepth) / 256, 2), 256, 0, stream>>>((uint32_t)n, m0, m1, c->eval_heap.get());
+	CU(cudaGetLastError());
+	evalm::k_pairwise_root<<<2, 1024, 0, stream>>>((uint32_t)n, c->eval_heap.get(), out_mse_ssim);
 	CU(cudaGetLastError());
 	return NSB_OK;
 }

@@ -14,6 +14,8 @@
 //                                           reference's float order (no JSON: the host keeps its own load / save)
 //   ngp_b200::render_to_cpu(...)        <- Testbed::render_to_cpu's sub-frame loop (python_api.cu:129-175) and copy back, over
 //                                           nsb_render_accumulate; the caller builds the sub-frames (nerfshop_b200/camera_path.py restates how)
+//   ngp_b200::reference_image, image_metrics <- scripts/run.py's --test_transforms block (run.py:215-302): read_image and the MSE / SSIM
+//                                           of a rendered frame on the device
 //
 // Errors become std::runtime_error, as CUDA_CHECK_THROW does in the reference (propagates to main.cu:252).
 #pragma once
@@ -297,6 +299,18 @@ inline void optimise_mesh_step(Context& ctx, const NsbMeshOptimise& p, uint32_t 
 inline void get_rgba_on_grid(Context& ctx, const NsbGridQuery& q, const float ray_dir[3], int32_t rgb_activation, int32_t density_activation, float* rgba_dev,
                              void* stream) {
 	check(nsb_rgba_on_grid(ctx.get(), &q, ray_dir, rgb_activation, density_activation, rgba_dev, stream), "nsb_rgba_on_grid");
+}
+
+// scripts/run.py's --test_transforms block (run.py:215-302) on device frames: read_image's ground truth from decoded 8-bit pixels (with
+// run.py's sRGB blend when srgb_blend), then compute_error("MSE") and compute_error("SSIM") of a rendered frame against it. mse_ssim_dev
+// (2 floats) stays on the device; the maps are optional (nullptr).
+inline void reference_image(Context& ctx, const uint8_t* pixels_dev, int32_t w, int32_t h, int32_t n_channels, bool srgb_blend, const float background[4],
+                            float* rgba_dev, void* stream) {
+	check(nsb_reference_image(ctx.get(), pixels_dev, w, h, n_channels, srgb_blend ? 1 : 0, background, rgba_dev, stream), "nsb_reference_image");
+}
+inline void image_metrics(Context& ctx, const float* image_dev, const float* ref_dev, int32_t w, int32_t h, float* mse_ssim_dev, void* stream,
+                          float* mse_map_dev = nullptr, float* ssim_map_dev = nullptr) {
+	check(nsb_image_metrics(ctx.get(), image_dev, ref_dev, w, h, mse_ssim_dev, mse_map_dev, ssim_map_dev, stream), "nsb_image_metrics");
 }
 
 #ifdef NSB_HOST_HAVE_CUDART

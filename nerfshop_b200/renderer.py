@@ -11,6 +11,8 @@
       save_density_grid_to_png / save_rgba_grid_to_png_sequence (marching_cubes.cu:898-1015); nerfshop_b200.slices writes the files
   NerfRenderer.render_accumulate / frame_to_rgba8 <- Testbed::render_to_cpu's sub-frame loop (python_api.cu:129-175) and scripts/run.py's
       8-bit video frames (write_image, scripts/common.py:122-178); nerfshop_b200.camera_path builds camera paths and videos on them
+  NerfRenderer.reference_image / image_metrics <- scripts/run.py's --test_transforms block (run.py:215-302): read_image's ground truth and
+      compute_error("MSE" / "SSIM") with their means; nerfshop_b200.evaluate scores test views and writes screenshots on them
 
 torch is used for device memory and streams only; every computation is a call into libnerfshop_b200.so.
 """
@@ -303,6 +305,36 @@ class NerfRenderer:
         s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
         abi.check(self.lib, self.lib.nsb_frame_to_rgba8(self.ctx, rgba.data_ptr(), W, H, float(exposure), int(n_channels), out.data_ptr(), s),
                   "nsb_frame_to_rgba8")
+        return out
+
+    # ---- image-quality metrics (scripts/run.py --test_transforms) ------------------------------------------------------------------
+    def reference_image(self, pixels, srgb_blend: bool = False, background=(0.0, 0.0, 0.0, 1.0), out=None, stream=None):
+        """nsb_reference_image: read_image's linear premultiplied RGBA (alpha 1 for RGB) from decoded 8-bit pixels, uint8 CUDA tensor
+        [H, W, 3 or 4]; srgb_blend: run.py's blend over `background` in sRGB (RGBA only). Returns float32 CUDA tensor [H, W, 4]. Stream-ordered."""
+        torch = _torch()
+        H, W, nc = pixels.shape
+        if out is None:
+            out = torch.empty((H, W, 4), dtype=torch.float32, device=torch.device("cuda", self.device))
+        bg = (C.c_float * 4)(*[float(v) for v in background])
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_reference_image(self.ctx, pixels.data_ptr(), W, H, nc, int(bool(srgb_blend)), bg, out.data_ptr(), s),
+                  "nsb_reference_image")
+        return out
+
+    def image_metrics(self, image, ref, out=None, mse_map=None, ssim_map=None, stream=None):
+        """nsb_image_metrics on two float32 CUDA tensors [H, W, 4] (the rendered frame, the ground truth): run.py's MSE and SSIM of the frame,
+        float32 CUDA tensor [2] = (MSE, SSIM), left on the device. mse_map / ssim_map: float32 CUDA tensors [H, W] to receive the maps, or
+        None. Stream-ordered."""
+        torch = _torch()
+        H, W = image.shape[0], image.shape[1]
+        if tuple(ref.shape[:2]) != (H, W):
+            raise ValueError(f"image_metrics: image {tuple(image.shape)} and ground truth {tuple(ref.shape)} differ in size")
+        if out is None:
+            out = torch.empty(2, dtype=torch.float32, device=torch.device("cuda", self.device))
+        s = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        abi.check(self.lib, self.lib.nsb_image_metrics(self.ctx, image.data_ptr(), ref.data_ptr(), W, H, out.data_ptr(),
+                                                       0 if mse_map is None else mse_map.data_ptr(), 0 if ssim_map is None else ssim_map.data_ptr(), s),
+                  "nsb_image_metrics")
         return out
 
     # ---- operator-level entry points ---------------------------------------------------------------------

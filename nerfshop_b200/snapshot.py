@@ -83,8 +83,7 @@ def _density_grid(blob: bytes) -> np.ndarray:
     raise abi.NsbError(f"density_grid_binary has {len(blob)} bytes: neither float32 x 5 x 128^3 (save_snapshot) nor fp16 x k x 128^3, k = 1..5 (export_snapshot)")
 
 
-def load_snapshot(path: str):
-    """-> (NsbModelDesc, params uint16[n], density_grid float32[5*128^3], aabb_scale)."""
+def _read(path: str) -> dict:
     import msgpack
 
     with open(path, "rb") as fh:
@@ -93,7 +92,22 @@ def load_snapshot(path: str):
         import zlib
 
         blob = zlib.decompress(blob, 15 + 32)
-    cfg = msgpack.unpackb(blob, raw=False)
+    return msgpack.unpackb(blob, raw=False)
+
+
+def load_dataset_transform(path: str):
+    """-> (scale, offset (3 floats), from_mitsuba): the snapshot's nerf.dataset members that NerfDataset::nerf_matrix_to_ngp reads
+    (nerf_loader.h:74-92), as load_snapshot restores them (json_binding.h:189-194). A snapshot without a dataset (export_snapshot's)
+    leaves the NerfDataset defaults (nerf_loader.h:49-55): 1, (0, 0, 0), false."""
+    ds = _read(path)["snapshot"].get("nerf", {}).get("dataset")
+    if ds is None:
+        return 1.0, (0.0, 0.0, 0.0), False
+    return float(ds["scale"]), tuple(float(v) for v in ds["offset"]), bool(ds["from_mitsuba"])
+
+
+def load_snapshot(path: str):
+    """-> (NsbModelDesc, params uint16[n], density_grid float32[5*128^3], aabb_scale)."""
+    cfg = _read(path)
     enc, net, rgb = cfg["encoding"], cfg["network"], cfg["rgb_network"]
     snap = cfg["snapshot"]
     if snap.get("params_type", "__half") != "__half":
