@@ -13,11 +13,15 @@ The absent dependencies (Eigen fork, tiny-cuda-nn, tinylogger, json, OpenGL) are
 oracle/ref_shim/ (our code, written for this purpose). tiny-cuda-nn's network itself (hash grid + MLPs) is NOT available:
 ref_driver.cpp's NerfNetwork calls back into a function pointer supplied by the test (the oracle's encode + MLP).
 
-Compiler flags: -ffp-contract=fast -mfma, so that gcc contracts a*b+c into FMAs inside expressions the way nvcc's default
+Compiler flags (GXX_KERNELS): -ffp-contract=fast -mfma, so that gcc contracts a*b+c into FMAs inside expressions the way nvcc's default
 -fmad=true does for the reference's device code (CMakeLists.txt:71-80 sets no --fmad=false). The two compilers' contraction
 rules are not guaranteed to coincide; tests/test_oracle_vs_ref.py reports every comparison as a count of differing values.
 
 The GPU box has no /root/reference: the .so is built here and travels with the repository snapshot (git-ignored).
+
+Every library of oracle/_ref (this module's two and those of the other oracle/ref_*_build.py) is built by build_library: its cut-outs
+(write_cutouts), one of the flag lists below plus its own include directories, and a rebuild whenever a file of dependencies() is newer.
+NSB_REF_KEEP_GEN=1 keeps the cut-outs (and nvcc's intermediate files) under oracle/_ref/gen*/ for inspection.
 """
 from __future__ import annotations
 
@@ -33,12 +37,24 @@ OUT_DIR = os.path.join(HERE, "_ref")
 LIB = os.path.join(OUT_DIR, "libnerfshop_ref.so")
 LIB_CUDA = os.path.join(OUT_DIR, "libnerfshop_ref_cuda.so")
 DRIVER_CUDA = os.path.join(HERE, "ref_driver_cuda.cu")
-COMMON = os.path.join(HERE, "ref_common.inl")
 SHIM = os.path.join(HERE, "ref_shim")
 DRIVER = os.path.join(HERE, "ref_driver.cpp")
+REF_INCLUDES = ["-I", os.path.join(REF, "include"), "-I", os.path.join(REF, "src")]
 
-# (reference file, [(kind, regex of the first line), ...]); kind "fn" = function definition (brace matched, a preceding
-# `template <...>` line is taken along), "stmt" = statement up to the terminating ';'
+_GXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
+# the compiler and the flags of each kind of build; a library adds its include directories, its driver and what else it names
+NVCC = [shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17",
+        "--extended-lambda", "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-shared", "-w"] + (
+        ["-ccbin", "/usr/bin/g++"] if os.path.exists("/usr/bin/g++") else [])
+# the reference's kernels on the CPU: OpenMP over the launch grid, and a*b+c contracted as nvcc's -fmad=true does
+GXX_KERNELS = [_GXX, "-std=c++17", "-O2", "-fPIC", "-shared", "-fopenmp", "-ffp-contract=fast", "-mfma", "-fno-fast-math",
+               "-Wno-deprecated-declarations", "-Wno-attributes", "-w"]
+# the reference's host code: its host build does not contract
+GXX_HOST = [_GXX, "-std=c++17", "-O2", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-w"]
+
+# {name: (reference file, [(kind, regex of the first line[, regex of the last line]), ...])}, written to name.inc by write_cutouts; kind
+# "fn" = function definition (brace matched, a preceding `template <...>` line is taken along), "stmt" = statement up to the terminating
+# ';', "range" = from the first line to the next line that matches the second regex
 EXTRACTS = {
     "testbed_nerf": ("src/testbed_nerf.cu", [
         ("stmt", r"^static constexpr uint32_t MARCH_ITER\b"),
@@ -164,7 +180,8 @@ def _strip_for_braces(line: str, in_block: bool):
     return "".join(out), in_block
 
 
-def cut(lines, kind, pattern):
+def cut(lines, kind, pattern, last=None):
+    """(first, last) index of the lines of one cut-out; its first line is the one line that matches pattern."""
     rx = re.compile(pattern)
     hits = [i for i, l in enumerate(lines) if rx.search(l)]
     if len(hits) != 1:
@@ -191,8 +208,12 @@ def cut(lines, kind, pattern):
             i += 1
         end = i
     elif kind == "range":
-        # ("range", first-line anchor, last-line anchor): statements out of the middle of a member whose surroundings cannot be compiled here
-        raise RuntimeError("range cuts take two anchors: use cut_range")
+        # statements out of the middle of a member whose surroundings cannot be compiled here
+        rx_last = re.compile(last)
+        ends = [i for i in range(start, len(lines)) if rx_last.search(lines[i])]
+        if not ends:
+            raise RuntimeError(f"anchor {last!r}: no match after line {start + 1}")
+        end = ends[0]
     else:
         i = start
         while ";" not in lines[i]:
@@ -201,98 +222,110 @@ def cut(lines, kind, pattern):
     return first, end
 
 
-def cut_range(lines, first_pattern, last_pattern):
-    a, b = re.compile(first_pattern), re.compile(last_pattern)
-    starts = [i for i, l in enumerate(lines) if a.search(l)]
-    if len(starts) != 1:
-        raise RuntimeError(f"anchor {first_pattern!r}: {len(starts)} matches (expected exactly 1)")
-    ends = [i for i in range(starts[0], len(lines)) if b.search(lines[i])]
-    if not ends:
-        raise RuntimeError(f"anchor {last_pattern!r}: no match after line {starts[0] + 1}")
-    return starts[0], ends[0]
-
-
-def extract_all(gen_dir: str):
-    os.makedirs(gen_dir, exist_ok=True)
+def write_cutouts(table, gen_dir: str, transform=lambda line: line):
+    """Writes each entry of a table shaped like EXTRACTS to gen_dir/name.inc: its cut-outs in order, each line passed through transform,
+    each behind a #line directive to where it lies in the reference. Returns the manifest lines (file:first-last, anchor)."""
     manifest = []
-    for name, (rel, items) in EXTRACTS.items():
+    for name, (rel, items) in table.items():
         path = os.path.join(REF, rel)
         with open(path, "r", encoding="utf-8", errors="replace") as fh:
             lines = fh.read().split("\n")
         parts = []
         for item in items:
-            kind, pattern = item[0], item[1]
-            a, b = cut_range(lines, item[1], item[2]) if kind == "range" else cut(lines, kind, pattern)
-            manifest.append(f"{rel}:{a + 1}-{b + 1}  {pattern}")
-            # the one mechanical rewrite: CUDA's launch syntax is not C++ (same kernel, same arguments, same grid)
-            body = [LAUNCH_RX.sub(r"nsb_launch(\2, \3, \1, ", l) for l in lines[a:b + 1]]
+            a, b = cut(lines, *item)
+            manifest.append(f"{rel}:{a + 1}-{b + 1}  {item[1]}")
+            body = [transform(l) for l in lines[a:b + 1]]
             parts.append(f"// ---- {rel}:{a + 1}-{b + 1} ----\n#line {a + 1} \"{path}\"\n" + "\n".join(body) + "\n")
         with open(os.path.join(gen_dir, name + ".inc"), "w") as fh:
             fh.write("\n".join(parts))
     return manifest
 
 
+def extract_all(gen_dir: str):
+    """EXTRACTS, with the one mechanical rewrite: CUDA's launch syntax is not C++ (same kernel, same arguments, same grid)."""
+    return write_cutouts(EXTRACTS, gen_dir, lambda line: LAUNCH_RX.sub(r"nsb_launch(\2, \3, \1, ", line))
+
+
 def available() -> bool:
     return os.path.isdir(os.path.join(REF, "src")) and os.path.exists(os.path.join(REF, "src", "testbed_nerf.cu"))
 
 
-def needs_build(lib: str = LIB, driver: str = DRIVER) -> bool:
-    if not os.path.exists(lib):
-        return True
-    t = os.path.getmtime(lib)
-    deps = [driver, COMMON, os.path.abspath(__file__), os.path.join(HERE, "..", "include", "nerfshop_b200.h")]
-    for root, _, files in os.walk(SHIM):
-        deps += [os.path.join(root, f) for f in files]
-    return any(os.path.getmtime(d) > t for d in deps)
+_INCLUDE_RX = re.compile(r'^\s*#\s*include\s*"([^"]+)"', re.M)
+
+
+def dependencies(driver: str, shims, module: str):
+    """The repository's files a library is built from: its driver and every file the driver's quoted #includes reach in the repository,
+    every file under its stand-in directories, this module and the library's own build module."""
+    deps, todo = set(), [os.path.abspath(driver)]
+    while todo:
+        path = todo.pop()
+        if path in deps:
+            continue
+        deps.add(path)
+        with open(path, "r", encoding="utf-8") as fh:
+            for inc in _INCLUDE_RX.findall(fh.read()):
+                inc = os.path.normpath(os.path.join(os.path.dirname(path), inc))
+                if os.path.isfile(inc):
+                    todo.append(inc)
+    for d in shims:
+        for root, _, files in os.walk(d):
+            deps.update(os.path.join(root, f) for f in files)
+    deps.update((os.path.abspath(__file__), os.path.abspath(module)))
+    return sorted(deps)
+
+
+def stale(lib: str, deps) -> bool:
+    return not os.path.exists(lib) or any(os.path.getmtime(d) > os.path.getmtime(lib) for d in deps)
+
+
+def build_library(lib: str, driver: str, gen_name: str, compile_cmd, cut, shims, module: str, force: bool = False):
+    """Builds one library of oracle/_ref unless it is newer than every file of dependencies(driver, shims, module): cut(gen) writes the
+    cut-outs into the fresh directory oracle/_ref/<gen_name>, compile_cmd(gen) is run, and the cut-outs (reference source) are deleted
+    unless NSB_REF_KEEP_GEN=1. Returns the library's path, or None when the reference's sources are absent and no prebuilt library
+    exists."""
+    if not available():
+        return lib if os.path.exists(lib) else None
+    if not force and not stale(lib, dependencies(driver, shims, module)):
+        return lib
+    gen = os.path.join(OUT_DIR, gen_name)
+    shutil.rmtree(gen, ignore_errors=True)
+    os.makedirs(gen)
+    cut(gen)
+    cmd = compile_cmd(gen)
+    keep = os.environ.get("NSB_REF_KEEP_GEN") == "1"
+    if keep and cmd[0] == NVCC[0]:
+        cmd += ["--keep", "--keep-dir", gen]
+    res = subprocess.run(cmd, capture_output=True, text=True)
+    if not keep:
+        shutil.rmtree(gen, ignore_errors=True)
+    if res.returncode != 0:
+        raise RuntimeError(f"oracle/_ref/{os.path.basename(lib)} build failed:\n" + res.stdout + res.stderr[-6000:])
+    return lib
 
 
 def build(force: bool = False, verbose: bool = False):
     """Returns the path of the library, or None when /root/reference is absent (GPU box) and no prebuilt library exists."""
-    if not available():
-        return LIB if os.path.exists(LIB) else None
-    if not force and not needs_build():
-        return LIB
-    gen = os.path.join(OUT_DIR, "gen")
-    shutil.rmtree(gen, ignore_errors=True)
-    manifest = extract_all(gen)
-    cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-    cmd = [cxx, "-std=c++17", "-O2", "-fPIC", "-shared", "-fopenmp", "-ffp-contract=fast", "-mfma", "-fno-fast-math",
-           "-Wno-deprecated-declarations", "-Wno-attributes", "-w",
-           "-I", SHIM, "-I", gen, "-I", os.path.join(REF, "include"), "-I", os.path.join(REF, "src"),
-           "-x", "c++", DRIVER, "-o", LIB]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    keep = os.environ.get("NSB_REF_KEEP_GEN") == "1"
-    if not keep:
-        shutil.rmtree(gen, ignore_errors=True)  # the cut-outs are reference source: they do not stay on disk
-    if res.returncode != 0:
-        raise RuntimeError("oracle/_ref build failed:\n" + res.stdout + res.stderr[-6000:])
-    with open(os.path.join(OUT_DIR, "MANIFEST.txt"), "w") as fh:
-        fh.write("reference functions compiled into libnerfshop_ref.so (file:first-last line, anchor)\n" + "\n".join(manifest) + "\n")
-    if verbose:
-        print("\n".join(manifest))
-    return LIB
+    manifest = []
+
+    def cut_and_record(gen):
+        manifest.extend(extract_all(gen))
+
+    lib = build_library(LIB, DRIVER, "gen", lambda gen: GXX_KERNELS + ["-I", SHIM, "-I", gen, *REF_INCLUDES, "-x", "c++", DRIVER, "-o", LIB],
+                        cut_and_record, [SHIM], __file__, force)
+    if manifest:  # compiled just now
+        with open(os.path.join(OUT_DIR, "MANIFEST.txt"), "w") as fh:
+            fh.write("reference functions compiled into libnerfshop_ref.so (file:first-last line, anchor)\n" + "\n".join(manifest) + "\n")
+        if verbose:
+            print("\n".join(manifest))
+    return lib
 
 
 def build_cuda(force: bool = False):
     """The same reference sources compiled by nvcc for sm_90a (oracle/ref_driver_cuda.cu): the reference's kernels and host loop
     run on the GPU. Returns the library path, or None when /root/reference is absent and no prebuilt library exists."""
-    if not available():
-        return LIB_CUDA if os.path.exists(LIB_CUDA) else None
-    if not force and not needs_build(LIB_CUDA, DRIVER_CUDA):
-        return LIB_CUDA
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    gen = os.path.join(OUT_DIR, "gen_cuda")
-    shutil.rmtree(gen, ignore_errors=True)
-    extract_all(gen)
-    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "--extended-lambda", "--expt-relaxed-constexpr",
-           "-Xcompiler", "-fPIC", "-shared", "-w"] + (["-ccbin", "/usr/bin/g++"] if os.path.exists("/usr/bin/g++") else []) + [
-           "-I", SHIM, "-I", gen, "-I", os.path.join(REF, "include"), "-I", os.path.join(REF, "src"), DRIVER_CUDA, "-o", LIB_CUDA]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if os.environ.get("NSB_REF_KEEP_GEN") != "1":
-        shutil.rmtree(gen, ignore_errors=True)
-    if res.returncode != 0:
-        raise RuntimeError("oracle/_ref CUDA build failed:\n" + res.stdout + res.stderr[-6000:])
-    return LIB_CUDA
+    return build_library(LIB_CUDA, DRIVER_CUDA, "gen_cuda",
+                         lambda gen: NVCC + ["-lineinfo", "-I", SHIM, "-I", gen, *REF_INCLUDES, DRIVER_CUDA, "-o", LIB_CUDA],
+                         extract_all, [SHIM], __file__, force)
 
 
 if __name__ == "__main__":

@@ -10,13 +10,11 @@ are deleted after the compile) and #included by oracle/ref_mesh_driver_cuda.cu:
                           extract_srgb_with_activation
 The reference's network (tiny-cuda-nn, absent) is not part of it: the tests run this repository's nsb_density / nsb_inference between
 the reference's kernels, as the render-path parity does. Stand-ins for the absent submodules: oracle/ref_shim/ and oracle/ref_shim_mesh/
-(filesystem/path.h, stb_image_write.h). Flags are ref_build.build_cuda's.
+(filesystem/path.h, stb_image_write.h). Flags: ref_build.NVCC.
 """
 from __future__ import annotations
 
 import os
-import shutil
-import subprocess
 
 from . import ref_build
 
@@ -27,60 +25,29 @@ SHIM = os.path.join(HERE, "ref_shim_mesh")
 
 EXTRACTS = {
     "marching_cubes_mesh": ("src/marching_cubes.cu", [
-        r"^Vector3i get_marching_cubes_res\(",
-        r"^__global__ void gen_vertices\(",
-        r"^__global__ void accumulate_1ring\(",
-        r"^__global__ void gen_faces\(",
-        r"^void compute_mesh_1ring\(",
-        r"^void marching_cubes_gpu\(",
-        r"^void save_mesh\(",
+        ("fn", r"^Vector3i get_marching_cubes_res\("),
+        ("fn", r"^__global__ void gen_vertices\("),
+        ("fn", r"^__global__ void accumulate_1ring\("),
+        ("fn", r"^__global__ void gen_faces\("),
+        ("fn", r"^void compute_mesh_1ring\("),
+        ("fn", r"^void marching_cubes_gpu\("),
+        ("fn", r"^void save_mesh\("),
     ]),
     "testbed_nerf_mesh": ("src/testbed_nerf.cu", [
-        r"^__global__ void generate_grid_samples_nerf_uniform\(",
-        r"^__global__ void grid_samples_half_to_float\(",
-        r"^__global__ void generate_nerf_network_inputs_from_positions\(",
-        r"^__global__ void extract_srgb_with_activation\(",
+        ("fn", r"^__global__ void generate_grid_samples_nerf_uniform\("),
+        ("fn", r"^__global__ void grid_samples_half_to_float\("),
+        ("fn", r"^__global__ void generate_nerf_network_inputs_from_positions\("),
+        ("fn", r"^__global__ void extract_srgb_with_activation\("),
     ]),
 }
 
 
-def _deps():
-    deps = [DRIVER, os.path.abspath(__file__)]
-    for d in (SHIM, ref_build.SHIM):
-        for root, _, files in os.walk(d):
-            deps += [os.path.join(root, f) for f in files]
-    return deps
-
-
 def build(force: bool = False):
     """Returns the library path, or None when /root/reference is absent and no prebuilt library exists."""
-    if not ref_build.available():
-        return LIB if os.path.exists(LIB) else None
-    if not force and os.path.exists(LIB) and all(os.path.getmtime(d) <= os.path.getmtime(LIB) for d in _deps()):
-        return LIB
-    gen = os.path.join(ref_build.OUT_DIR, "gen_mesh")
-    shutil.rmtree(gen, ignore_errors=True)
-    os.makedirs(gen, exist_ok=True)
-    for name, (rel, anchors) in EXTRACTS.items():
-        with open(os.path.join(ref_build.REF, rel), "r", encoding="utf-8", errors="replace") as fh:
-            lines = fh.read().split("\n")
-        parts = []
-        for anchor in anchors:
-            a, b = ref_build.cut(lines, "fn", anchor)
-            parts.append(f"#line {a + 1} \"{os.path.join(ref_build.REF, rel)}\"\n" + "\n".join(lines[a:b + 1]) + "\n")
-        with open(os.path.join(gen, name + ".inc"), "w") as fh:
-            fh.write("\n".join(parts))
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--extended-lambda", "--expt-relaxed-constexpr",
-           "-Xcompiler", "-fPIC", "-shared", "-w"] + (["-ccbin", "/usr/bin/g++"] if os.path.exists("/usr/bin/g++") else []) + [
-           "-I", SHIM, "-I", ref_build.SHIM, "-I", gen, "-I", os.path.join(ref_build.REF, "include"), "-I", os.path.join(ref_build.REF, "src"),
-           DRIVER, "-o", LIB]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if os.environ.get("NSB_REF_KEEP_GEN") != "1":
-        shutil.rmtree(gen, ignore_errors=True)
-    if res.returncode != 0:
-        raise RuntimeError("oracle/_ref mesh build failed:\n" + res.stdout + res.stderr[-6000:])
-    return LIB
+    return ref_build.build_library(
+        LIB, DRIVER, "gen_mesh",
+        lambda gen: ref_build.NVCC + ["-I", SHIM, "-I", ref_build.SHIM, "-I", gen, *ref_build.REF_INCLUDES, DRIVER, "-o", LIB],
+        lambda gen: ref_build.write_cutouts(EXTRACTS, gen), [SHIM, ref_build.SHIM], __file__, force)
 
 
 if __name__ == "__main__":
